@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rays/sec of NeuRAD's volumetric-rendering hot path on B200 (BASELINE.json metric).
+"""bench.py -- rays/sec of NeuRAD's volumetric-rendering hot path on H100 (BASELINE.json metric).
 
 A "step" is one pass of the hot path over one synthetic PandaSet-shaped time step (BASELINE config 2): 6 x 1920x1080
 pinhole cameras traced at NeuRAD's render stride ([1::3,1::3] -> 6 x 230 400 rays) and one 64-beam x 1800-azimuth lidar
@@ -7,7 +7,7 @@ sweep (115 200 rays) = 1 497 600 traced rays, reference default grids / MLPs (ra
 Metric as the reference defines it: rays / time between device synchronisations (nerfstudio/pipelines/ad_pipeline.py:
 198-208, 296-304); only TRACED rays are counted (the reference counts the 9x larger full-resolution pixel grid).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 Two timed arms per run:
   value  device-resident inputs: ray generation + ONE `get_nff_outputs` launch pair over the whole time step.
@@ -85,7 +85,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not a measured figure)"
 
 
 RENDER_KERNEL_SOURCES = ("b200nerf.cu", "nff_device.h", "nff_lane.h", "nff_params.h", "simt.h", "tc_mlp.cuh")
@@ -100,6 +100,16 @@ def kernel_sources_sha() -> str:
         h.update(name.encode())
         h.update(open(os.path.join(ROOT, "neurad-studio_b200", "csrc", name), "rb").read())
     return h.hexdigest()[:16]
+
+
+def traffic_capture(path: str):
+    """(capture, source) of the render pair's counter capture at `path` if taken at the current kernel sources, else (None, why)."""
+    if not os.path.exists(path):
+        return None, "no hardware-counter capture of the render kernels is committed: not reported"
+    tj = json.load(open(path))
+    if tj.get("kernel_sources_sha") != kernel_sources_sha():
+        return None, f"{os.path.basename(path)} was captured for other kernel sources (sha mismatch): not reported"
+    return tj, tj.get("source")
 
 
 class ClockSampler:
@@ -420,13 +430,15 @@ def main():
     ap.add_argument("--gather", default="p2p", choices=["p2p", "nccl"],
                     help="N>1: p2p = render epilogue stores rows into every peer's buffer over NVLink (default); "
                          "nccl = all_gather_into_tensor after the render")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (a fixed seeded sample of rays) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     args.warmup = max(args.warmup, 3)
     # every rank (also the single one at N = 1: the API arm's pinned buffers and launch latencies otherwise depend on which
-    # socket the scheduler happened to start the process on -- 38.7 vs 44.4 ms per e2e step between two fresh boxes)
+    # socket the scheduler happened to start the process on)
     numa = bind_to_gpu_numa_node(local_rank) if args.impl == "b200" else {"node": None, "cpus": None}
 
     import neurad_studio_b200 as nsb
@@ -436,7 +448,7 @@ def main():
         "metric": "rays/sec (camera+lidar)", "unit": "rays/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "rays_per_step_per_gpu": 6 * CAM_RAYS + 115200, "tables": "fp32, main 8x2^22x4 + proposal 6x2^20x1 (U(-1,1))",
-                   "l2": "inputs larger than L2 (560 MB of tables, 300 MB of outputs per step); no explicit flush", "kernel": "ray-per-lane, 2-D tile walk (image_width=640), tcgen05 3xTF32 MLPs", "parallelism": f"ray-shard dp{world}" + ("" if world == 1 else f", gather={args.gather}")},
+                   "l2": "inputs larger than L2 (560 MB of tables, 300 MB of outputs per step); no explicit flush", "kernel": "ray-per-lane, 2-D tile walk (image_width=640), wgmma 3xTF32 MLPs", "parallelism": f"ray-shard dp{world}" + ("" if world == 1 else f", gather={args.gather}")},
     }
 
     if args.impl == "reference":
@@ -524,14 +536,20 @@ def main():
     if rank == 0:
         sampler.start()
     step.launches = 0
-    ms = timed(lambda: step.run_device(True), args.steps)
+    last = {}
+
+    def timed_step():
+        last["out"] = step.run_device(True)
+
+    ms = timed(timed_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     launches = step.launches // args.steps
     kern_ms = sorted(a.elapsed_time(b) for a, b in step.kernel_events)
     kern_ms = sum(kern_ms) / len(kern_ms)
     step.e2e_launches = 0
     # B200_E2E_DECODER_STREAM=1: the API arm pipelines image i's rgb decoder (side stream) under image i + 1's render
-    # (NeuRADModel.set_decoder_stream; +2 % in back-to-back A/B runs).  Off by default: two of three full bench runs with it
-    # showed a much slower e2e arm (44 / 61 ms per step instead of 38; the single-stream arm never did), not understood yet.
+    # (NeuRADModel.set_decoder_stream).  Off by default: its effect on the e2e arm has not been measured on an H100.
     dec_stream = os.environ.get("B200_E2E_DECODER_STREAM", "0") != "0"
     if dec_stream:
         model.set_decoder_stream(torch.cuda.Stream(device=dev))
@@ -624,12 +642,12 @@ def main():
         mac_per_ray = 48 * 32 + 4 * 50176 + 32 * 288 + 9 * (4 * 50176 + 3 * 32)
         tf = 2.0 * mac_per_ray * step.n_cam / (d_ms * 1e-3) / 1e12
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-        tpeak = float(peaks.get("bf16_tflops_sustained", 1443.2))
+        tpeak = float(peaks.get("bf16_tflops_sustained", 989.0))  # fallback: H100 SXM data sheet, dense bf16
         dec_line = {"value": step.n * args.steps / (ms_dec * 1e-3), "unit": "rays/s", "ms_per_step": ms_dec / args.steps,
                     "decoder_ms": d_ms, "decoder_camera_rays_per_s": step.n_cam / (d_ms * 1e-3), "gpu_launches_decoder": 10,
                     "roofline": {"bound": "tensor", "achieved": tf, "executed": 3 * tf, "peak": tpeak, "unit": "TFLOP/s",
                                  "frac": tf / tpeak, "frac_executed": 3 * tf / tpeak,
-                                 "note": "achieved = algorithmic 4.04 MFLOP/camera ray; executed = 3x (bf16 hi/lo split: three MMAs per product for fp32-level accuracy); peak = measured sustained dense bf16"},
+                                 "note": "achieved = algorithmic 4.04 MFLOP/camera ray; executed = 3x (bf16 hi/lo split: three MMAs per product for fp32-level accuracy); peak = measured sustained dense bf16 if MEASURED_PEAKS.json exists, else the data-sheet 989"},
                     "what": "render step + NeuRADModel.rgb_decoder on the 6 feature images (6x360x640x48 -> 6x1080x1920x3 rgb)"}
     # BASELINE configs[2] / configs[3]: secondary legs with the same roofline block, N = 1
     extras = {}
@@ -647,16 +665,11 @@ def main():
         return
     roof = roofline_block(step.n, kern_ms, "nff_sample_lane_kernel + nff_shade_lane_kernel (one render)")
     roof["bound_note"] = ("HBM is the CONTRACTUAL bound (algorithmic gather bytes / measured copy bandwidth); physically the pair is "
-                          "issue-bound: L1/L2 absorb ~94 % of the gathers (traffic << algorithmic bytes), see `limiter`")
-    traffic_file = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(traffic_file):
-        tj = json.load(open(traffic_file))
-        if tj.get("kernel_sources_sha") == kernel_sources_sha():
-            roof["traffic"] = tj.get("dram_bytes_per_launch")
-            roof["limiter"] = tj.get("limiter")
-            roof["traffic_source"] = tj.get("source")
-        else:
-            roof["traffic_source"] = "profiles/traffic.json was captured for other kernel sources (sha mismatch): not reported"
+                          "issue-bound when L1/L2 absorb most of the gathers (traffic << algorithmic bytes), see `limiter`")
+    tj, roof["traffic_source"] = traffic_capture(os.path.join(ROOT, "profiles", "traffic.json"))
+    if tj is not None:
+        roof["traffic"] = tj.get("dram_bytes_per_launch")
+        roof["limiter"] = tj.get("limiter")
     line = dict(base, value=value, ms_per_step=ms / args.steps, clocks=clocks, gpu_launches=launches,
                 e2e={"value": e2e_value, "unit": "rays/s", "h2d_bytes_per_step": step.h2d_bytes, "d2h_bytes_per_step": step.d2h_bytes,
                      "ms_per_step": ms_e2e / args.steps, "host_buffers_verified": bool(e2e_ok), "gpu_launches": e2e_launches,
@@ -688,6 +701,25 @@ def main():
         import torch.distributed as dist
 
         dist.destroy_process_group()
+
+
+DUMP_ROWS = 1 << 17  # rays kept per output array by --dump-outputs: 53 floats x 128 Ki rays = 28 MB in all
+
+
+def dump_outputs(path: str, out: dict):
+    """The render step's outputs ([n_rays, width] each) at the same seeded random sample of rays, as float32 .npy files."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    n = next(iter(out.values())).shape[0]
+    rows = None
+    if n > DUMP_ROWS:
+        g = torch.Generator().manual_seed(0)
+        rows = torch.randperm(n, generator=g)[:DUMP_ROWS].sort().values
+    np.save(os.path.join(path, "ray_index.npy"), (rows if rows is not None else torch.arange(n)).numpy().astype(np.float64))
+    for k, v in sorted(out.items()):
+        v = v.detach().float().cpu()
+        np.save(os.path.join(path, f"{k}.npy"), (v[rows] if rows is not None else v).numpy())
 
 
 def secondary_legs(be, cfg, dev, steps, timed) -> dict:

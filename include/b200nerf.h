@@ -1,4 +1,4 @@
-/* b200nerf.h -- C ABI of libb200nerf.so, the sm_100a backend of NeuRAD's volumetric-rendering hot path.
+/* b200nerf.h -- C ABI of libb200nerf.so, the sm_90a backend of NeuRAD's volumetric-rendering hot path.
  *
  * The reference (georghess/neurad-studio) has no FFI of its own: its backend seam is the string flag
  * `NeuRADModelConfig.implementation` (nerfstudio/models/neurad.py:146) that selects tiny-cuda-nn or torch
@@ -231,10 +231,10 @@ int b200nerf_hashgrid_fwd(b200nerf_ctx* ctx, const b200nerf_grid_desc* desc, con
 int b200nerf_sh4_fwd(b200nerf_ctx* ctx, const float* dirs, float* out, int64_t n_points, void* stream);
 
 /* MLP.forward (field_components/mlp.py:142-183; the tcnn FullyFusedMLP role, mlp.py:103-113) for NeuRAD's tiny
- * MLPs on the tcgen05 tensor cores with the 3xTF32 split (fp32-level accuracy): x [n_rows, in_dim] -> y [n_rows,
+ * MLPs on the wgmma tensor cores with the 3xTF32 split (fp32-level accuracy): x [n_rows, in_dim] -> y [n_rows,
  * out_dims[n_layers-1]]; ReLU between layers, none at the output.  `weights_host` / `biases_host` are HOST arrays
  * of `n_layers` device pointers in nn.Linear layout ([out,in] / [out]; biases_host or its entries may be NULL).
- * Limits: 1..3 layers, every width <= 64 (<= 48: 48-column TMEM tile; wider, e.g. BASELINE config 1's 32 -> 64 -> 4:
+ * Limits: 1..3 layers, every width <= 64 (<= 48: 48-column tile; wider, e.g. BASELINE config 1's 32 -> 64 -> 4:
  * 64-column tile). */
 int b200nerf_mlp_fwd(b200nerf_ctx* ctx, const float* x, int64_t n_rows, int in_dim, int n_layers,
                      const float* const* weights_host, const float* const* biases_host, const int* out_dims_host,
@@ -249,7 +249,7 @@ int b200nerf_mlp_fwd_train(b200nerf_ctx* ctx, const float* x, int64_t n_rows, in
 /* Input gradient of one Linear layer of those MLPs (autograd of F.linear + ReLU, mlp.py:170-178):
  *   dx [n_rows, dx_dim] = dy [n_rows, dy_dim] @ weight_t^T,   weight_t = the layer's nn.Linear weight TRANSPOSED, [dx_dim, dy_dim]
  * and, when relu_z [n_rows, dx_dim] (the pre-activation that fed this layer through ReLU) is given, dx *= (relu_z > 0).
- * Same tcgen05 3xTF32 operator as b200nerf_mlp_fwd. */
+ * Same wgmma 3xTF32 operator as b200nerf_mlp_fwd. */
 int b200nerf_mlp_dgrad(b200nerf_ctx* ctx, const float* dy, int64_t n_rows, int dy_dim, const float* weight_t, int dx_dim,
                        const float* relu_z, float* dx, void* stream);
 
@@ -281,7 +281,7 @@ int b200nerf_neurad_encoding_fwd(b200nerf_ctx* ctx, int field, const float* mean
  *         [geo_embedding | SHEncoding(4)(get_normalized_directions(d))]
  *   tail: feature [P,G] = geo_embedding + mlp_feature_out; sdf [P] = geo_out[:,0]; alpha [P] = sigmoid(-sdf * beta)
  *         with beta = |sdf_to_density.beta| + 1e-4 (model_components/utils.py:29-41).  sdf / alpha may be NULL.
- * The MLPs themselves run through b200nerf_mlp_fwd (tcgen05). */
+ * The MLPs themselves run through b200nerf_mlp_fwd (wgmma). */
 int b200nerf_field_mid_fwd(b200nerf_ctx* ctx, const float* geo_out, const float* directions, int64_t n_points,
                            int geo_feat_dim, float* mlp_feature_in, void* stream);
 int b200nerf_field_tail_fwd(b200nerf_ctx* ctx, const float* geo_out, const float* mlp_feature_out, int64_t n_points,
@@ -367,15 +367,14 @@ int b200nerf_field_heads_bwd(b200nerf_ctx* ctx, const float* geo_out, const floa
 /* MLP backward pieces (field_components/mlp.py:142-178).  For layer l with input X (a hidden pre-activation Z when
  * relu_x != 0, so act = ReLU) and output gradient dY:
  *   b200nerf_linear_wgrad : dweight [out,in] += dY^T act(X), dbias [out] += sum dY            (widths <= 64)
- *   dX = dY W: b200nerf_mlp_dgrad (above; tcgen05, ReLU mask fused), or b200nerf_mlp_fwd with the transposed weight and
+ *   dX = dY W: b200nerf_mlp_dgrad (above; wgmma, ReLU mask fused), or b200nerf_mlp_fwd with the transposed weight and
  *   b200nerf_relu_bwd     : dZ *= (Z > 0) in place. */
 int b200nerf_linear_wgrad(b200nerf_ctx* ctx, const float* x, const float* dy, int64_t n_rows, int in_dim, int out_dim,
                           int relu_x, float* dweight, float* dbias, void* stream);
 int b200nerf_relu_bwd(b200nerf_ctx* ctx, const float* z, float* dz, int64_t n, void* stream);
-/* EXPERIMENTAL twin of b200nerf_linear_wgrad on the tcgen05 tensor cores (split-K GEMM, output rows in the TMEM lanes,
- * 48 input rows per MMA chunk, 3xTF32): same arguments and semantics.  Written after the round's GPU budget was spent; the
- * CUDA-core operator stays the default until this one has been validated and timed on a B200 (a tensor-core barrier
- * time-out raises the b200nerf_check_status flag instead of hanging). */
+/* EXPERIMENTAL twin of b200nerf_linear_wgrad on the wgmma tensor cores (split-K GEMM, output rows = the rows of a
+ * 128-row wgmma tile, 48 input rows per MMA chunk, 3xTF32): same arguments and semantics.  The CUDA-core operator stays
+ * the default until this one has been timed. */
 int b200nerf_linear_wgrad_tc(b200nerf_ctx* ctx, const float* x, const float* dy, int64_t n_rows, int in_dim, int out_dim,
                              int relu_x, float* dweight, float* dbias, void* stream);
 
@@ -403,8 +402,8 @@ int b200nerf_lidar_carving_mask(b200nerf_ctx* ctx, const float* bins_e, const ui
 
 /* Kernel variant used by b200nerf_nff_render_fwd:
  *   2 (default) ray-per-lane mapping (a warp = 32 adjacent rays at one sample index: coherent gathers), MLPs on the
- *     tcgen05 tensor cores with the 3xTF32 split (fp32-level accuracy, |err| ~1e-6 relative);
- *   1 warp-per-ray mapping, tcgen05 MLPs;   0 warp-per-ray mapping, CUDA-core fp32 FFMA MLPs. */
+ *     wgmma tensor cores with the 3xTF32 split (fp32-level accuracy, |err| ~1e-6 relative);
+ *   1 warp-per-ray mapping, wgmma MLPs;   0 warp-per-ray mapping, CUDA-core fp32 FFMA MLPs. */
 int b200nerf_set_mlp_mode(b200nerf_ctx* ctx, int mode);
 
 /* Synchronises with the device and reports (then clears) the device-side failure flag that kernels raise instead
@@ -504,7 +503,7 @@ int64_t b200nerf_rgb_decode_workspace_bytes(int batch, int height, int width);
 
 /* The camera half of NeuRADModel.decode_features (models/neurad.py:359-366): features [batch, height, width, in_dim]
  * (= the row-major ray order of b200nerf_nff_render_fwd's `features` output, so no permute is needed) ->
- * rgb [batch, 3*height, 3*width, 3].  impl 0: the 7x7 convolutions run as implicit GEMMs on the tcgen05 tensor cores
+ * rgb [batch, 3*height, 3*width, 3].  impl 0: the 7x7 convolutions run as implicit GEMMs on the wgmma tensor cores
  * (bf16 hi/lo split, fp32 accumulate, fp32-level accuracy), operands moved by the TMA engine; impl 2: the same with
  * per-thread 16-byte asynchronous copies instead of TMA; impl 1: the same pipeline on the CUDA cores in fp32 (slow
  * cross-check of the same op). */

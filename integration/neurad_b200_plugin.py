@@ -1,4 +1,4 @@
-"""Reference-side plugin: NeuRAD with the B200-native NFF backend, registered through nerfstudio's own plugin mechanism.
+"""Reference-side plugin: NeuRAD with the H100-native NFF backend, registered through nerfstudio's own plugin mechanism.
 
 This file is imported INSIDE an installation of the reference (georghess/neurad-studio): it subclasses the reference's
 `NeuRADModel` / `NeuRADModelConfig` (nerfstudio/models/neurad.py:97-165) and exports a `MethodSpecification`
@@ -10,7 +10,7 @@ This file is imported INSIDE an installation of the reference (georghess/neurad-
 `eval_setup` use it like any other method.  What changes for the reference: `get_nff_outputs` -- the whole of
 `neurad.py:368-421` in eval mode -- becomes one call into libb200nerf.so (ray sampling, both proposal rounds, main field,
 compositing, appearance), `get_outputs_for_camera_ray_bundle` renders an image in ONE call instead of the 32 768-ray chunk
-loop (`neurad.py:650-659`), and in eval mode the rgb / lidar decoders run on the library's tcgen05 kernels.  Parameters stay
+loop (`neurad.py:650-659`), and in eval mode the rgb / lidar decoders run on the library's wgmma kernels.  Parameters stay
 the reference's own `nn.Parameter`s in the `implementation="torch"` layout (bound zero-copy by pointer), so checkpoints,
 optimizers and `state_dict()` are untouched.  Training (grad mode) falls through to the reference's own module walk.
 
@@ -68,7 +68,7 @@ def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
 
 @dataclass
 class B200NeuRADModelConfig(NeuRADModelConfig):
-    """NeuRADModelConfig with the B200 backend.  `implementation` stays "torch": the parameters then have the layout the
+    """NeuRADModelConfig with the H100 backend.  `implementation` stays "torch": the parameters then have the layout the
     library binds by pointer (fp32 `[L*T, F]` tables, nn.Linear MLPs), and checkpoints interchange with the reference's
     torch mode."""
 
@@ -80,7 +80,7 @@ class B200NeuRADModelConfig(NeuRADModelConfig):
 
 
 class B200NeuRADModel(NeuRADModel):
-    """`NeuRADModel` whose eval-mode NFF path is the sm_100a library."""
+    """`NeuRADModel` whose eval-mode NFF path is the sm_90a library."""
 
     config: B200NeuRADModelConfig
 
@@ -146,7 +146,7 @@ class B200NeuRADModel(NeuRADModel):
 
     def decode_features(self, features: Tensor, patch_size: Tuple[int, int], is_lidar: Optional[Tensor] = None,
                         intensity_for_cam: bool = False):
-        """neurad.py:337-366.  Eval mode: lidar MLP and camera CNN on the library's tcgen05 kernels (channels-last in and
+        """neurad.py:337-366.  Eval mode: lidar MLP and camera CNN on the library's wgmma kernels (channels-last in and
         out, so the reference's two permutes disappear); training: the reference's modules (BatchNorm statistics, autograd)."""
         if self.training or torch.is_grad_enabled() or not self.config.b200_decoders:
             return super().decode_features(features, patch_size, is_lidar, intensity_for_cam)
@@ -182,7 +182,7 @@ def _make_spec() -> MethodSpecification:
     ref = cfg.pipeline.model
     fields = {k: v for k, v in vars(ref).items() if k not in ("_target", "implementation", "eval_num_rays_per_chunk")}
     cfg.pipeline.model = B200NeuRADModelConfig(**fields)
-    return MethodSpecification(config=cfg, description="NeuRAD with the B200-native (sm_100a) neural-feature-field backend")
+    return MethodSpecification(config=cfg, description="NeuRAD with the H100-native (sm_90a) neural-feature-field backend")
 
 
 spec = _make_spec()

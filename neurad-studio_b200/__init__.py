@@ -1,4 +1,4 @@
-"""neurad-studio_b200 -- B200-native (sm_100a) backend for NeuRAD's volumetric-rendering hot path.
+"""neurad-studio_b200 -- H100-native (sm_90a) backend for NeuRAD's volumetric-rendering hot path.
 
 Import as ``neurad_studio_b200`` (the top-level ``neurad_studio_b200.py`` shim maps the importable name onto
 this directory, whose on-disk name carries a hyphen).

@@ -95,7 +95,7 @@ class DensityFn(Function):
 
 
 class MlpFn(Function):
-    """MLP.forward (ReLU hidden layers, linear output) on the tcgen05 operator; args: x, then weight_0, bias_0, ..."""
+    """MLP.forward (ReLU hidden layers, linear output) on the wgmma operator; args: x, then weight_0, bias_0, ..."""
 
     @staticmethod
     @_fwd

@@ -1,4 +1,4 @@
-"""Host side of the sm_100a NeuRAD backend: owns a `b200nerf_ctx`, feeds it torch CUDA tensors by pointer and
+"""Host side of the sm_90a NeuRAD backend: owns a `b200nerf_ctx`, feeds it torch CUDA tensors by pointer and
 launches the kernels on torch's current stream.  PyTorch is plumbing here (device memory, streams); all compute
 is in libb200nerf.so.  There is no CPU path: constructing a `B200Backend` without a CUDA device raises.
 """
@@ -47,7 +47,7 @@ class B200Backend:
 
     def __init__(self, device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("neurad_studio_b200 requires a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("neurad_studio_b200 requires a CUDA (sm_90a) device; there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("neurad_studio_b200 runs on CUDA devices only")
@@ -329,7 +329,7 @@ class B200Backend:
 
     def mlp_fwd(self, x: torch.Tensor, weights: Sequence[torch.Tensor], biases: Optional[Sequence[Optional[torch.Tensor]]] = None,
                 want_hidden: bool = False):
-        """MLP.forward (field_components/mlp.py:142-183) on the tcgen05 tensor cores (3xTF32): ReLU hidden
+        """MLP.forward (field_components/mlp.py:142-183) on the wgmma tensor cores (3xTF32): ReLU hidden
         activations, no output activation.  weights[i] is nn.Linear's [out_i, in_i].  `want_hidden` (training): returns
         (y, [pre-activation of hidden layer l, [n_rows, out_l]]) -- what the backward needs, stored by the same launch."""
         xs = self._dev(x).reshape(-1, x.shape[-1])
@@ -351,7 +351,7 @@ class B200Backend:
 
     def set_mlp_mode(self, mode: str):
         """Kernel variant of render(): 'split' (default) ray-per-lane in two kernels -- sampling at 32 warps/SM, then
-        shading with tcgen05 MLPs; 'lane' the same code as one fused kernel; 'tc' warp-per-ray + tcgen05 MLPs
+        shading with wgmma MLPs; 'lane' the same code as one fused kernel; 'tc' warp-per-ray + wgmma MLPs
         (3xTF32); 'ffma' warp-per-ray + CUDA-core fp32 MLPs."""
         self._check(self.lib.b200nerf_set_mlp_mode(self._h, {"ffma": 0, "tc": 1, "lane": 2, "split": 3}[mode]))
 
@@ -475,8 +475,8 @@ class B200Backend:
 
     def field_forward(self, mean: torch.Tensor, std: torch.Tensor, times: torch.Tensor, directions: torch.Tensor,
                       flip: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        """NeuRADField.forward (fields/neurad_field.py:128-152) on gaussians: encoding -> mlp_geo (tcgen05) ->
-        [geo_embedding | SH] -> mlp_feature (tcgen05) -> residual, sdf, alpha.  Five launches, all ours:
+        """NeuRADField.forward (fields/neurad_field.py:128-152) on gaussians: encoding -> mlp_geo (wgmma) ->
+        [geo_embedding | SH] -> mlp_feature (wgmma) -> residual, sdf, alpha.  Five launches, all ours:
         {"feature" [N,S,G], "sdf" [N,S,1], "alpha" [N,S,1]}."""
         n, s = mean.shape[0], mean.shape[1]
         enc = self.neurad_encoding(FIELD_MAIN, mean, std, times, directions, flip=flip)
@@ -612,7 +612,7 @@ class B200Backend:
     def linear_wgrad(self, x: torch.Tensor, dy: torch.Tensor, relu_x: bool, dweight: torch.Tensor, dbias: Optional[torch.Tensor],
                      impl: Optional[str] = None) -> None:
         """dweight [out,in] += dY^T act(X); dbias [out] += sum dY (act = ReLU when X is a hidden pre-activation).
-        impl "cuda" (default: CUDA cores, GPU-validated) or "tc" (experimental tcgen05 split-K twin; also selected by the
+        impl "cuda" (default: CUDA cores, GPU-validated) or "tc" (experimental wgmma split-K twin; also selected by the
         environment variable B200NERF_WGRAD=tc)."""
         xs, ds = self._dev(x), self._dev(dy)
         impl = impl or os.environ.get("B200NERF_WGRAD", "cuda")
@@ -621,7 +621,7 @@ class B200Backend:
                        self._stream))
 
     def mlp_dgrad(self, dy: torch.Tensor, weight: torch.Tensor, relu_z: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """dX = dY W of one Linear layer (weight = nn.Linear's [out, in]) on the tcgen05 operator; with `relu_z` (the
+        """dX = dY W of one Linear layer (weight = nn.Linear's [out, in]) on the wgmma operator; with `relu_z` (the
         pre-activation that fed the layer through ReLU) the result is masked by (relu_z > 0) in the same launch."""
         g = self._dev(dy).reshape(-1, dy.shape[-1]).contiguous()
         wt = self._dev(weight).t().contiguous()  # [in, out]
@@ -641,7 +641,7 @@ class B200Backend:
                 dweights: Sequence[Optional[torch.Tensor]], dbiases: Sequence[Optional[torch.Tensor]], need_dx: bool = True,
                 hidden: Optional[Sequence[torch.Tensor]] = None) -> Optional[torch.Tensor]:
         """MLP.forward backward (field_components/mlp.py:142-178): accumulates into dweights[l] / dbiases[l] (entries may
-        be None) and returns dL/dx.  Hidden pre-activations are recomputed with prefix forward passes (tcgen05); dX = dY W
+        be None) and returns dL/dx.  Hidden pre-activations are recomputed with prefix forward passes (wgmma); dX = dY W
         runs through the same tensor-core operator with the transposed weight; dW through linear_wgrad."""
         x2 = self._dev(x).reshape(-1, x.shape[-1])
         nl = len(weights)
@@ -792,7 +792,7 @@ class B200Backend:
 
     def rgb_decode(self, features: torch.Tensor, impl: str = "tc", out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Camera half of NeuRADModel.decode_features (neurad.py:359-366): features [B,H,W,C] (or [H,W,C]) ->
-        rgb [B,3H,3W,3].  impl "tc": tcgen05 implicit-GEMM convolutions with TMA operand loads; "tc_ldgsts": the same
+        rgb [B,3H,3W,3].  impl "tc": wgmma implicit-GEMM convolutions with TMA operand loads; "tc_ldgsts": the same
         with per-thread cp.async loads; "ref": CUDA-core fp32 cross-check."""
         f = self._dev(features)
         if f.dim() == 3:

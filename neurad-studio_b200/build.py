@@ -1,4 +1,4 @@
-"""Build libb200nerf.so (sm_100a) in-tree with nvcc.  No JIT cache: the built .so travels with the repo."""
+"""Build libb200nerf.so (sm_90a) in-tree with nvcc.  No JIT cache: build() writes the .so next to the package sources."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libb200nerf.so")
 SOURCES = ["b200nerf.cu"]
 HEADERS = ["nff_device.h", "nff_lane.h", "tc_mlp.cuh", "rgb_decoder.cuh", "nff_modules.h", "modules.cuh", "nff_params.h", "simt.h", os.path.join("..", "..", "include", "b200nerf.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-shared",
 ]

@@ -1,4 +1,4 @@
-// b200nerf.cu -- kernels + C ABI of libb200nerf.so (sm_100a).  See include/b200nerf.h for the contract.
+// b200nerf.cu -- kernels + C ABI of libb200nerf.so (sm_90a).  See include/b200nerf.h for the contract.
 #include <cuda_runtime.h>
 
 #include <cstdio>
@@ -45,7 +45,7 @@ struct b200nerf_ctx {
   int act_alloc_actors = 0, act_alloc_times = 0;  // sizes the actor arrays are currently allocated for
   int layout = 0;    // 0: torch-mode grids (b200nerf_set_field_grids); 1: tiny-cuda-nn layout (b200nerf_set_field_grids_tcnn)
   int field_layout[3] = {0, 0, 0};
-  int mlp_mode = 3;  // 3 = ray-per-lane in two kernels (sampling | shading + tcgen05), 2 = the same as one fused kernel, 1 = warp-per-ray + tcgen05 (3xTF32), 0 = warp-per-ray + CUDA-core fp32 FFMA
+  int mlp_mode = 3;  // 3 = ray-per-lane in two kernels (sampling | shading + wgmma), 2 = the same as one fused kernel, 1 = warp-per-ray + wgmma (3xTF32), 0 = warp-per-ray + CUDA-core fp32 FFMA
   float* d_lane_scratch = nullptr;
   int lane_ctas = 0;
   unsigned* d_minmax = nullptr;      // [2] ordered-bit min / max of the depth steps (DepthRenderer "expected" clip)
@@ -69,7 +69,7 @@ struct b200nerf_ctx {
   // NeuRADModel.rgb_decoder (rgb_decoder.cuh): folded / re-laid-out parameters owned by the context
   bool have_rgb_decoder = false;
   int dec_in_dim = 0;
-  unsigned char* d_dec_wimg[8] = {};  // [49][hi|lo] bf16 UMMA B tiles per 7x7 conv
+  unsigned char* d_dec_wimg[8] = {};  // [49][hi|lo] bf16 GMMA B tiles per 7x7 conv
   float* d_dec_wf32[8] = {};          // [49][ci][co] fp32 (CUDA-core reference kernel)
   float* d_dec_bias = nullptr;        // [8][32] folded conv + BN biases
   float* d_dec_small = nullptr;       // in conv w [32*in] b [32] | convT w [32*32*9] b [32] | out conv w [3*32] b [3]
@@ -105,6 +105,7 @@ int make_grid(const b200nerf_grid_desc* d, const float* table, Grid* g) {
 #ifndef NFF_WARPS
 #define NFF_WARPS 8
 #endif
+constexpr int kSmemMaxOptIn = 227 * 1024;  // dynamic shared memory a CTA may opt in to on sm_90
 constexpr int kRenderWarps = NFF_WARPS;  // warps (= rays in flight) per CTA; 16 warps/SM at <=128 registers
 
 // CUDA-core MLP variant (exact fp32 FFMA): the reference/fallback numerics mode.
@@ -122,44 +123,28 @@ __global__ void __launch_bounds__(WARPS * 32, 16 / WARPS) nff_render_kernel(cons
     render_ray(P, *ws, mlp, ray, true);
 }
 
-// Tensor-core MLP variant (tcgen05 + TMEM, 3xTF32): each group of 4 warps forms one 128-row tile.
+// Tensor-core MLP variant (wgmma, 3xTF32): each group of 4 warps (a warp group) forms one 128-row tile.
 using WarpSharedTc = WarpSharedT<kNff>;
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 16 / WARPS) nff_render_tc_kernel(const __grid_constant__ RenderParams P) {
   static_assert(WARPS % 4 == 0 && WARPS <= 16, "warp groups of 4");
   extern __shared__ __align__(128) unsigned char smem_tc[];
-  unsigned char* smem_raw = smem_tc;
-  TcShared* tcs = reinterpret_cast<TcShared*>(smem_raw);
-  constexpr int kTcBytes = (sizeof(TcShared) + 127) / 128 * 128;
+  TcShared* tcs = reinterpret_cast<TcShared*>(smem_tc);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
-  WarpSharedTc* ws = reinterpret_cast<WarpSharedTc*>(smem_raw + kTcBytes) + warp;
+  WarpSharedTc* ws = reinterpret_cast<WarpSharedTc*>(smem_tc + tc_smem_bytes(WARPS * 32)) + warp;
   tc_stage_weights(*tcs, P.main_mlp_nn, threadIdx.x, WARPS * 32);
-  tc::fence_async_smem();
-  constexpr uint32_t kCols = kTcTileCols * (WARPS / 4);
-  if (warp == 0) tc::tmem_alloc(&tcs->tmem_base, kCols);
-  if (threadIdx.x == 0)
-    for (int g = 0; g < WARPS / 4; ++g) tc::mbar_init(&tcs->bar[g], 1);
-  tc::fence_before_sync();
+  tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
-  tc::fence_after_sync();
   MlpTc mlp;
   mlp.t = tcs;
-  mlp.tile_base = __shfl_sync(0xffffffffu, tcs->tmem_base, 0) + (uint32_t)(group * kTcTileCols);
-  mlp.lane_base = mlp.tile_base + ((uint32_t)(32 * (warp & 3)) << 16);
-  mlp.bar = &tcs->bar[group];
-  mlp.parity = 0;
+  mlp.stage = reinterpret_cast<float*>(smem_tc + kTcBytes) + group * kTcStageFloats;
   mlp.bar_id = 1 + group;
-  mlp.issuer = (warp & 3) == 0;
-  mlp.status = P.status;
   const int64_t stride = (int64_t)gridDim.x * WARPS;
   for (int64_t base = (int64_t)blockIdx.x * WARPS; base < P.n_rays; base += stride) {
     const int64_t ray = base + warp;
     const bool active = ray < P.n_rays;
     render_ray(P, *ws, mlp, active ? ray : P.n_rays - 1, active);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tcs->tmem_base, kCols);
 }
 
 
@@ -201,11 +186,11 @@ __device__ __forceinline__ bool lane_unit_ray(const RenderParams& P, int64_t uni
 // 32x16 tile when the caller passes image_width, else 32 consecutive rays); patches are numbered tile by tile, so consecutive
 // patches are spatial neighbours.  Whole tiles (16 patches = one per warp) are taken grid-stride, tile k * gridDim + blockIdx,
 // for as many FULL rounds as there are -- all resident CTAs then work on adjacent tiles, which keeps their common working
-// set of grid cells compact in L2 (giving every CTA one long contiguous range instead cost 4 % on the 1.5 M-ray batch:
-// profiles/r02_ab_work_distribution_v1.txt).  The last, partial round is split evenly over ALL CTAs at patch granularity
+// set of grid cells compact in L2 (giving every CTA one long contiguous range instead puts far-apart regions in flight, which
+// thrashes L2).  The last, partial round is split evenly over ALL CTAs at patch granularity
 // (sampling: round-robin over a CTA's warps, there is no CTA-level synchronisation at all; shading: over its 128-ray warp
-// groups, one tensor-core tile = 4 consecutive patches).  With whole 512-ray CTA units a 230 400-ray image is 460 units on
-// 148 (x2) resident CTAs: a few SMs got 4 units where the others got 3 and the launch lasted 4 / 3.1 of its balanced time.
+// groups, one tensor-core tile = 4 consecutive patches).  With whole 512-ray CTA units a 230 400-ray image is 460 units, which
+// no count of resident CTAs (132 SMs on an H100) divides evenly: the SMs with one unit more would set the launch time.
 __device__ __forceinline__ int64_t lane_patches(const RenderParams& P) {
   return P.rays.image_width > 0 ? lane_units(P) * (kLaneThreads / 32) : (P.n_rays + 31) / 32;
 }
@@ -215,8 +200,8 @@ __device__ __forceinline__ bool lane_patch_ray(const RenderParams& P, int64_t pa
   return lane_unit_ray(P, patch / kPatchesPerUnit, (int)(patch % kPatchesPerUnit) * 32 + lane_, ray_out);
 }
 
-// Two-stage variant of the ray-per-lane path.  Stage 1 (sampling: both proposal rounds) needs neither TMEM nor shared
-// memory and fits 64 registers, so it runs at 32 warps/SM with the whole 228 KB as L1; stage 2 (main field + MLPs +
+// Two-stage variant of the ray-per-lane path.  Stage 1 (sampling: both proposal rounds) needs no shared memory and fits
+// 64 registers, so it runs at 32 warps/SM with the SM's whole 256 KB L1/shared array as L1; stage 2 (main field + MLPs +
 // compositing) is the tensor-core kernel at 16 warps/SM.  The hand-over is 33 spacing edges per ray ([edge][ray],
 // 132 B/ray) -- still nothing per-sample in HBM.
 #ifndef NFF_SAMPLE_CTAS
@@ -259,32 +244,20 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
                                                                                       const float* __restrict__ handoff) {
   extern __shared__ __align__(128) unsigned char smem_shade[];
   TcShared* tcs = reinterpret_cast<TcShared*>(smem_shade);
-  constexpr int kTcBytes = (sizeof(TcShared) + 127) / 128 * 128;
-  float* geo_park = reinterpret_cast<float*>(smem_shade + kTcBytes);
+  float* geo_park = reinterpret_cast<float*>(smem_shade + tc_smem_bytes(kLaneThreads));
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
   tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
-  tc::fence_async_smem();
-  constexpr uint32_t kCols = kTcTileCols * (kLaneThreads / 128);
-  if (warp == 0) tc::tmem_alloc(&tcs->tmem_base, kCols);
-  if (tid == 0)
-    for (int g = 0; g < kLaneThreads / 128; ++g) tc::mbar_init(&tcs->bar[g], 1);
-  tc::fence_before_sync();
+  tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
-  tc::fence_after_sync();
   MlpLaneTc mlp;
   mlp.core.t = tcs;
-  mlp.core.tile_base = __shfl_sync(0xffffffffu, tcs->tmem_base, 0) + (uint32_t)(group * kTcTileCols);
-  mlp.core.lane_base = mlp.core.tile_base + ((uint32_t)(32 * (warp & 3)) << 16);
-  mlp.core.bar = &tcs->bar[group];
-  mlp.core.parity = 0;
+  mlp.core.stage = reinterpret_cast<float*>(smem_shade + kTcBytes) + group * kTcStageFloats;
   mlp.core.bar_id = 1 + group;
-  mlp.core.issuer = (warp & 3) == 0;
-  mlp.core.status = P.status;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
   mlp.geo_park = NFF_PANEL_GLOBAL ? sc.panel : geo_park;
   mlp.sh_tcnn = LAYOUT;
   // a warp group (one 128-row tensor-core tile) renders 4 consecutive patches; the groups of a CTA only meet at the two
-  // block barriers around the loop, inside it they synchronise among their own 4 warps (named barriers, mbarriers).
+  // block barrier before the loop, inside it they synchronise among their own 4 warps (named barriers).
   // Full rounds sweep adjacent tiles like the sampling kernel; the partial last round is dealt out group-unit by group-unit.
   constexpr int kPPU = kLaneThreads / 32;
   const int64_t n_patches = lane_patches(P);
@@ -306,9 +279,6 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
     const LaneRay R = lane_ray_setup(P, sc, tid, ray);
     shade_ray_lane<MlpLaneTc, LAYOUT>(P, sc, R, mlp, tid, ray, active, handoff + ray, P.n_rays);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tcs->tmem_base, kCols);
 }
 
 // Ray-per-lane variant (nff_lane.h), single fused kernel: a warp = 32 adjacent rays at the same sample index.
@@ -316,27 +286,15 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_
                                                                           float* __restrict__ scratch) {
   extern __shared__ __align__(128) unsigned char smem_lane[];
   TcShared* tcs = reinterpret_cast<TcShared*>(smem_lane);
-  constexpr int kTcBytes = (sizeof(TcShared) + 127) / 128 * 128;
-  float* geo_park = reinterpret_cast<float*>(smem_lane + kTcBytes);
+  float* geo_park = reinterpret_cast<float*>(smem_lane + tc_smem_bytes(kLaneThreads));
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
   tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
-  tc::fence_async_smem();
-  constexpr uint32_t kCols = kTcTileCols * (kLaneThreads / 128);
-  if (warp == 0) tc::tmem_alloc(&tcs->tmem_base, kCols);
-  if (tid == 0)
-    for (int g = 0; g < kLaneThreads / 128; ++g) tc::mbar_init(&tcs->bar[g], 1);
-  tc::fence_before_sync();
+  tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
-  tc::fence_after_sync();
   MlpLaneTc mlp;
   mlp.core.t = tcs;
-  mlp.core.tile_base = __shfl_sync(0xffffffffu, tcs->tmem_base, 0) + (uint32_t)(group * kTcTileCols);
-  mlp.core.lane_base = mlp.core.tile_base + ((uint32_t)(32 * (warp & 3)) << 16);
-  mlp.core.bar = &tcs->bar[group];
-  mlp.core.parity = 0;
+  mlp.core.stage = reinterpret_cast<float*>(smem_lane + kTcBytes) + group * kTcStageFloats;
   mlp.core.bar_id = 1 + group;
-  mlp.core.issuer = (warp & 3) == 0;
-  mlp.core.status = P.status;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
   mlp.geo_park = NFF_PANEL_GLOBAL ? sc.panel : geo_park;
   for (int64_t unit = blockIdx.x; unit < lane_units(P); unit += gridDim.x) {
@@ -344,9 +302,6 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_
     const bool active = lane_unit_ray(P, unit, tid, &ray);
     render_ray_lane(P, sc, mlp, tid, ray, active);
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tcs->tmem_base, kCols);
 }
 
 // NeuRADModel.decode_features, lidar half (models/neurad.py:350-357): one thread per ray.
@@ -741,8 +696,8 @@ __global__ void pack_linear_kernel(const float* __restrict__ w, const float* __r
 
 
 // MLP.forward (field_components/mlp.py:142-183) for NeuRAD's tiny MLPs on the tensor cores: up to 3 Linear layers,
-// ReLU between them, in/out widths <= 48.  One CTA = one 128-row tile at a time (grid-stride), activations in TMEM,
-// weights in shared memory (see tc_mlp.cuh).
+// ReLU between them, in/out widths <= 64.  One CTA (one warp group) = one 128-row tile at a time (grid-stride), each
+// layer a wgmma tile product through a shared-memory stage, weights in shared memory (see tc_mlp.cuh).
 struct MlpArgs {
   const float* w[3];
   const float* b[3];
@@ -750,6 +705,7 @@ struct MlpArgs {
   int k_real[3], n_real[3], k_pad[3], n_pad[3];
   int smem_off[3];  // float offsets of each layer's (hi) tile; lo follows at +n_pad*k_pad
   int bias_off;
+  int mma_off;    // [128][tc::stage_pitch(kTcKMax)] stage of the tensor-core layers
   int stage_off;  // 2 x [128][max(kTcKMax, kTcNMax) + 1] row tiles (input rows in / output rows out, double buffered)
   float* hidden_pre[2];  // training: pre-activation rows [n_rows, n_real[l]] of hidden layer l, or NULL
   const float* relu_mask;  // backward: rows [n_rows, out_dim] of a pre-activation Z; the output is multiplied by (Z > 0), or NULL
@@ -758,31 +714,23 @@ template <int kTcKMax, int kTcNMax>
 __global__ void __launch_bounds__(128) mlp_tc_kernel(const MlpArgs a, const float* __restrict__ x, float* __restrict__ y,
                                                      int64_t n_rows, int* __restrict__ status) {
   extern __shared__ __align__(128) float sm_mlp[];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(8) uint64_t bar;
-  using Cols = tc::TileCols<kTcKMax, kTcNMax>;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int tid = threadIdx.x;
   for (int l = 0; l < a.n_layers; ++l) {
     float* hi = sm_mlp + a.smem_off[l];
     tc::stage_b_tile(hi, hi + a.n_pad[l] * a.k_pad[l], a.w[l], a.n_real[l], a.k_real[l], a.n_pad[l], a.k_pad[l], tid, 128);
     for (int i = tid; i < kTcNMax; i += 128) sm_mlp[a.bias_off + l * kTcNMax + i] = (i < a.n_real[l] && a.b[l]) ? a.b[l][i] : 0.f;
   }
-  tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  if (warp == 0) tc::tmem_alloc(&tmem_base_s, 256);
-  if (tid == 0) tc::mbar_init(&bar, 1);
-  tc::fence_before_sync();
+  tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_s, 0);
-  const uint32_t lane_base = tmem_base + ((uint32_t)(32 * (warp & 3)) << 16);
-  uint32_t parity = 0;
+  float* mma_stage = sm_mlp + a.mma_off;
+  constexpr int kMmaPitch = tc::stage_pitch(kTcKMax);
   const int out_dim = a.n_real[a.n_layers - 1];
   // Rows travel through shared-memory tiles with an odd pitch: the CTA's 128 rows are one contiguous block of global
   // memory, moved with coalesced accesses by all threads, while thread = row reads its own row from shared memory
   // without bank conflicts.  (Thread = row straight from global memory touches 32 different lines per load instruction:
   // 48 loads + 48 stores x 32 wavefronts made the LSU the limit.)  The NEXT tile's rows are fetched with cp.async into
-  // the other buffer while this tile goes through the layers: with 8 warps per SM (TMEM allows two CTAs) nothing else
-  // would hide the DRAM latency (ncu: 12 % warps active, 60 % of the stall samples on the long scoreboard).
+  // the other buffer while this tile goes through the layers: with 8 warps per SM (two CTAs) nothing else
+  // would hide the DRAM latency.
   constexpr int kPitch = (kTcKMax > kTcNMax ? kTcKMax : kTcNMax) + 1;
   float* stage0 = sm_mlp + a.stage_off;
   float* mask_tile = stage0 + 2 * 128 * kPitch;  // [128 * out_dim], present when a.relu_mask
@@ -826,32 +774,24 @@ __global__ void __launch_bounds__(128) mlp_tc_kernel(const MlpArgs a, const floa
 #pragma unroll
     for (int k = 0; k < kTcKMax; ++k) v[k] = (row < n_rows && k < a.in_dim) ? stage[tid * kPitch + k] : 0.f;
     for (int l = 0; l < a.n_layers; ++l) {
-      tc::store_a<kTcKMax>(lane_base, 0, v, a.k_pad[l]);
-      tc::wait_st();
-      tc::fence_before_sync();
-      __syncthreads();
-      if (warp == 0) {  // converged warp, one elected lane issues (see tc::issue_layer)
-        tc::fence_after_sync();
-        const float* hi = sm_mlp + a.smem_off[l];
-        tc::issue_layer<kTcKMax>(tmem_base, Cols::d, hi, hi + a.n_pad[l] * a.k_pad[l], a.k_pad[l], a.n_pad[l], &bar);
+      const float* hi = sm_mlp + a.smem_off[l];
+      const float* lo = hi + a.n_pad[l] * a.k_pad[l];
+      auto sync = [] { __syncthreads(); };
+      float d[kTcNMax];
+      switch (a.n_pad[l]) {  // the MMA's N is an immediate: one instantiation per padded width (host: multiple of 16)
+        case 16: tc::tile_layer<kTcKMax, 16>(mma_stage, kMmaPitch, v, a.k_pad[l], hi, lo, d, sync); break;
+        case 32: tc::tile_layer<kTcKMax, 32>(mma_stage, kMmaPitch, v, a.k_pad[l], hi, lo, d, sync); break;
+        case 48: tc::tile_layer<kTcKMax, 48>(mma_stage, kMmaPitch, v, a.k_pad[l], hi, lo, d, sync); break;
+        default:
+          if constexpr (kTcNMax > 48) tc::tile_layer<kTcKMax, 64>(mma_stage, kMmaPitch, v, a.k_pad[l], hi, lo, d, sync);
+          break;
       }
-      if (!tc::mbar_wait(&bar, parity)) atomicExch(status, 1);
-      parity ^= 1u;
-      tc::fence_after_sync();
-      uint32_t d[kTcNMax];
-      tc::tmem_ld16(lane_base + Cols::d, d);
-      if (a.n_pad[l] > 16) tc::tmem_ld16(lane_base + Cols::d + 16, d + 16);
-      if (a.n_pad[l] > 32) tc::tmem_ld16(lane_base + Cols::d + 32, d + 32);
-      if constexpr (kTcNMax > 48) {
-        if (a.n_pad[l] > 48) tc::tmem_ld16(lane_base + Cols::d + 48, d + 48);
-      }
-      tc::wait_ld();
       const float* bias = sm_mlp + a.bias_off + l * kTcNMax;
       const bool last = l == a.n_layers - 1;
       float* hid = last ? nullptr : a.hidden_pre[l];  // warp-uniform
 #pragma unroll
       for (int k = 0; k < kTcNMax; ++k) {
-        float o = k < a.n_pad[l] ? __uint_as_float(d[k]) + bias[k] : 0.f;
+        float o = k < a.n_pad[l] ? d[k] + bias[k] : 0.f;
         if (hid && k < a.n_real[l]) stage[tid * kPitch + k] = o;  // (the input rows were consumed before this layer's barrier)
         v[k] = last ? o : fmaxf(o, 0.f);
       }
@@ -901,9 +841,6 @@ __global__ void __launch_bounds__(128) mlp_tc_kernel(const MlpArgs a, const floa
     }
     __syncthreads();  // this buffer is the prefetch target of the next iteration
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 256);
 }
 
 // Cameras._generate_rays_from_coords, pinhole + rolling shutter (cameras/cameras.py:633-667,793-798,898-969)
@@ -1077,8 +1014,8 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
   DeviceGuard g(device_ordinal);
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device_ordinal));
-  if (prop.major < 10)
-    return fail(B200NERF_ERR_UNSUPPORTED, "libb200nerf is built for sm_100a only (found sm_" +
+  if (prop.major != 9 || prop.minor != 0)  // sm_90a code (wgmma, TMA) loads on compute capability 9.0 only
+    return fail(B200NERF_ERR_UNSUPPORTED, "libb200nerf is built for sm_90a only (found sm_" +
                                               std::to_string(prop.major) + std::to_string(prop.minor) + ")");
   b200nerf_ctx* c = new (std::nothrow) b200nerf_ctx();
   REQUIRE(c != nullptr, "out of host memory");
@@ -1087,17 +1024,17 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
   CUDA_TRY(cudaFuncSetAttribute(nff_render_kernel<kRenderWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 (int)((kMainMlpFloats * 4 + 15) / 16 * 16 + kRenderWarps * sizeof(WarpShared))));
   CUDA_TRY(cudaFuncSetAttribute(nff_render_tc_kernel<kRenderWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)((sizeof(TcShared) + 127) / 128 * 128 + kRenderWarps * sizeof(WarpSharedTc))));
+                                (int)(tc_smem_bytes(kRenderWarps * 32) + kRenderWarps * sizeof(WarpSharedTc))));
   CUDA_TRY(cudaMalloc((void**)&c->d_status, sizeof(int)));
   CUDA_TRY(cudaMemset(c->d_status, 0, sizeof(int)));
   CUDA_TRY(cudaFuncSetAttribute(nff_render_lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)((sizeof(TcShared) + 127) / 128 * 128 + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
   c->lane_ctas = c->sm_count * (kLaneCtasPerSm > NFF_SAMPLE_CTAS ? kLaneCtasPerSm : NFF_SAMPLE_CTAS);
   CUDA_TRY(cudaMalloc((void**)&c->d_lane_scratch, sizeof(float) * lane_scratch_floats_per_cta() * c->lane_ctas));
   CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)((sizeof(TcShared) + 127) / 128 * 128 + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
   CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)((sizeof(TcShared) + 127) / 128 * 128 + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
   CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<0>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));  // all L1
   CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
   CUDA_TRY(cudaMalloc((void**)&c->d_minmax, 2 * sizeof(unsigned)));
@@ -1442,7 +1379,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
   if (c->mlp_mode == 3) {
     // sampling kernel -> [33][rays] spacing edges -> shading kernel; bundles larger than the hand-over buffer are
     // rendered in slices (whole 16-row tile bands when an image_width hint is given)
-    const size_t smem = (sizeof(TcShared) + 127) / 128 * 128 + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
+    const size_t smem = tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
     int64_t slice = c->handoff_rays;
     if (rays->image_width > 0) {
       const int64_t band = (int64_t)rays->image_width * (kLaneThreads / 32);
@@ -1474,7 +1411,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       }
     }
   } else if (c->mlp_mode == 2) {
-    const size_t smem = (sizeof(TcShared) + 127) / 128 * 128 + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
+    const size_t smem = tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
     int64_t need = (n_rays + kLaneThreads - 1) / kLaneThreads;
     if (rays->image_width > 0) {
       const int64_t W = rays->image_width, H = (n_rays + W - 1) / W;
@@ -1483,7 +1420,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
     int lane_blocks = (int)(need < c->lane_ctas ? need : c->lane_ctas);
     nff_render_lane_kernel<<<lane_blocks, kLaneThreads, smem, st>>>(P, c->d_lane_scratch);
   } else if (c->mlp_mode == 1) {
-    const size_t smem = (sizeof(TcShared) + 127) / 128 * 128 + WARPS * sizeof(WarpSharedTc);
+    const size_t smem = tc_smem_bytes(WARPS * 32) + WARPS * sizeof(WarpSharedTc);
     nff_render_tc_kernel<WARPS><<<blocks, WARPS * 32, smem, st>>>(P);
   } else {
     const size_t smem = (kMainMlpFloats * 4 + 15) / 16 * 16 + WARPS * sizeof(WarpShared);
@@ -1553,13 +1490,15 @@ static int mlp_fwd_impl(b200nerf_ctx* c, const float* x, int64_t n_rows, int in_
   a.relu_mask = relu_mask;
   // NeuRAD's own MLPs (<= 48 wide) use the 48-column tile; wider ones (config 1's 32 -> 64 -> 4) the 64-column tile
   const int tile_w = wmax <= 48 ? 48 : kWide;
-  a.stage_off = off + 3 * tile_w;
+  a.mma_off = off + 3 * tile_w;
+  a.stage_off = a.mma_off + 128 * tc::stage_pitch(tile_w);
   size_t smem = sizeof(float) * (a.stage_off + 2 * 128 * (tile_w + 1) + (relu_mask ? 128 * out_dims_host[n_layers - 1] : 0));
   // function attributes are per device: one flag per context (several contexts, one per GPU, may share the process)
+  REQUIRE(smem <= (size_t)kSmemMaxOptIn, "MLP too wide: its weights and row tiles exceed a CTA's shared memory");
   bool& attr_set = c->mlp_attr_set;
   if (!attr_set) {
-    CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel<48, 48>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-    CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 172 * 1024));
+    CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel<48, 48>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMaxOptIn));
+    CUDA_TRY(cudaFuncSetAttribute(mlp_tc_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMaxOptIn));
     attr_set = true;
   }
   int64_t tiles = (n_rows + 127) / 128;
@@ -1896,7 +1835,8 @@ int b200nerf_linear_wgrad_tc(b200nerf_ctx* c, const float* x, const float* dy, i
   DeviceGuard g(c->device);
   const int64_t chunks = (n_rows + kWgTcRows - 1) / kWgTcRows;
   const int grid = (int)(chunks < (int64_t)c->sm_count ? chunks : (int64_t)c->sm_count);
-  linear_wgrad_tc_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(x, dy, n_rows, in_dim, out_dim, relu_x, dweight, dbias, c->d_status);
+  CUDA_TRY(cudaFuncSetAttribute(linear_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgTcSmemBytes));
+  linear_wgrad_tc_kernel<<<grid, 128, kWgTcSmemBytes, (cudaStream_t)stream>>>(x, dy, n_rows, in_dim, out_dim, relu_x, dweight, dbias);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -2088,7 +2028,7 @@ int b200nerf_rgb_decode_fwd(b200nerf_ctx* c, const float* features, int batch, i
                             void* workspace, int64_t workspace_bytes, int impl, void* stream) {
   REQUIRE(c, "ctx is NULL");
   REQUIRE(batch >= 0 && height >= 0 && width >= 0, "negative image shape");
-  REQUIRE(impl >= 0 && impl <= 2, "impl: 0 = tcgen05 + TMA loads, 1 = CUDA-core fp32 cross-check, 2 = tcgen05 + LDGSTS loads");
+  REQUIRE(impl >= 0 && impl <= 2, "impl: 0 = wgmma + TMA loads, 1 = CUDA-core fp32 cross-check, 2 = wgmma + LDGSTS loads");
   if (!c->have_rgb_decoder) return fail(B200NERF_ERR_STATE, "set_rgb_decoder was not called");
   if (batch == 0 || height == 0 || width == 0) return 0;
   REQUIRE(features && rgb && workspace, "NULL argument");
@@ -2183,7 +2123,7 @@ int b200nerf_set_param_stream(b200nerf_ctx* c, void* stream) {
 
 int b200nerf_set_mlp_mode(b200nerf_ctx* c, int mode) {
   REQUIRE(c, "ctx is NULL");
-  REQUIRE(mode >= 0 && mode <= 3, "render mode: 0 = warp-per-ray + CUDA-core fp32, 1 = warp-per-ray + tcgen05, 2 = ray-per-lane + tcgen05, 3 = ray-per-lane in two kernels (sampling, shading)");
+  REQUIRE(mode >= 0 && mode <= 3, "render mode: 0 = warp-per-ray + CUDA-core fp32, 1 = warp-per-ray + wgmma, 2 = ray-per-lane + wgmma, 3 = ray-per-lane in two kernels (sampling, shading)");
   c->mlp_mode = mode;
   return 0;
 }

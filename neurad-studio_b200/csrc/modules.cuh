@@ -47,7 +47,7 @@ struct EncodingArgs {
 // samples at a time.  F = 4 (main field) / F = 1 (proposal fields), at most 8 levels: a sample's feature row stays in
 // registers (neurad_encode_point_t), and the warp's 32 rows -- one contiguous block of `features` -- go out through a
 // shared-memory tile with an odd pitch so that the global stores are coalesced (lane = row wrote 32 different lines per
-// store instruction: 85 % LSU-wavefront utilisation, profiles/r02_ncu_train_kernels.txt).
+// store instruction).
 template <int F>
 __global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_fwd_kernel(const FieldGrids fg, const Actors A,
                                                                               const EncodingArgs a) {
@@ -417,7 +417,7 @@ __global__ void relu_bwd_kernel(const float* __restrict__ z, float* __restrict__
 // Weight / bias gradient of one Linear layer of the tiny MLPs: dW[o][i] += sum_p dY[p][o] * act(X[p][i]),
 // db[o] += sum_p dY[p][o]; K, N <= 64.  A CTA walks row tiles of 32, stages X / dY in shared memory and keeps its
 // share of the N*K outputs in registers (first version on the CUDA cores: K = rows is the long GEMM dimension here and
-// the output is at most 64 x 64; a split-K tcgen05 version is the next step for this operator).
+// the output is at most 64 x 64; a split-K wgmma version is the next step for this operator).
 constexpr int kWgradThreads = 256, kWgradRows = 32;
 // global -> shared copy of one [rows][W] row block into a tile of pitch ld (>= W, pad columns zero-filled), asynchronous
 // (cp.async: no registers, completion through commit / wait groups).  16-byte copies when the rows are whole quads.
@@ -440,7 +440,7 @@ __global__ void __launch_bounds__(kWgradThreads) linear_wgrad_kernel(const float
                                                                      int64_t n_rows, int K, int N, int relu_x,
                                                                      float* __restrict__ dW, float* __restrict__ db) {
   // two stages: the next tile's rows are in flight while this one is multiplied (a CTA that waited for its own loads
-  // spent half its time at the first shared-memory store after them: profiles/r02_ncu_train_kernels.txt)
+  // would stall at the first shared-memory store after them)
   __shared__ __align__(16) float xs2[2][kWgradRows * 64];
   __shared__ __align__(16) float dys2[2][kWgradRows * 64];
   const int ldx = (K + 3) & ~3, ldy = (N + 3) & ~3;  // rows padded to whole quads (pad columns zero)
@@ -543,16 +543,17 @@ __global__ void lidar_carving_mask_kernel(const float* __restrict__ bins_e, cons
   mask[i] = m;
 }
 
-// ---------------------------------------------------------------------------------- weight gradient on tcgen05
+// ---------------------------------------------------------------------------------- weight gradient on wgmma
 // dW[o][i] += sum_r dY[r][o] * act(X[r][i]) as a split-K GEMM on the tensor cores, built from the pieces of
-// mlp_tc_kernel (tc_mlp.cuh): the 128 TMEM lanes are the OUTPUT rows o (lanes >= N hold zeros), a chunk of 48 input
-// rows r is the K dimension.  Per chunk, thread o gathers its column dY[r0..r0+48)[o] (coalesced across threads for a
-// fixed r) into A (TMEM, hi/lo TF32 split), the CTA stages X^T for the chunk as the B tile (shared memory, K-major
-// no-swizzle layout, hi/lo), and one elected lane issues 6 k-steps x 3 MMAs that ACCUMULATE into the same TMEM columns
-// across all chunks of the CTA.  At the end every thread reads its row of D and adds it to global dW (one atomic per
-// output and CTA).  EXPERIMENTAL: written after the round's GPU budget was spent; b200nerf_linear_wgrad (CUDA cores) stays
-// the default until this variant has been validated and timed on a B200.
-constexpr int kWgTcRows = 48;  // rows per chunk = K of the chunk's MMAs (TileCols K_MAX)
+// mlp_tc_kernel (tc_mlp.cuh): the tile's 128 rows are the OUTPUT rows o, a chunk of 48 input rows r is K.  Per chunk
+// thread o stages its column dY[r0..r0+48)[o] as A, the CTA stages X^T as the B tile (N padded to 64), and the
+// accumulators stay in registers across the CTA's chunks; at the end one atomic per output and CTA adds them to dW.  EXPERIMENTAL: b200nerf_linear_wgrad (CUDA cores) stays the default until this variant has been timed.
+constexpr int kWgTcRows = 48;  // rows per chunk = K of the chunk's MMAs
+constexpr int kWgTcN = 64;     // MMA N: the layer's input width, padded
+constexpr int kWgTcPitch = tc::stage_pitch(kWgTcN);
+// [hi | lo] B tile (24 KB), then the A stage (26 KB); at the end the D rows (pitch kWgTcPitch) reuse the whole buffer
+constexpr size_t kWgTcSmemBytes = sizeof(float) * (2 * kWgTcN * kWgTcRows + 128 * tc::stage_pitch(kWgTcRows));
+static_assert(kWgTcSmemBytes >= 128 * kWgTcPitch * sizeof(float), "D rows do not fit");
 __device__ __forceinline__ void wg_stage_xt(float* hi, float* lo, const float* __restrict__ x, int64_t r0, int64_t n_rows, int K, int n_pad,
                                             bool relu_x, int tid, int nthreads) {
   // B(n = i, k = r) = act(X[r0 + r][i]); i runs fastest so that the global reads are contiguous
@@ -566,49 +567,18 @@ __device__ __forceinline__ void wg_stage_xt(float* hi, float* lo, const float* _
     lo[off] = v - h;
   }
 }
-// tc::issue_layer with a caller-chosen accumulate flag for the first k-step (chunks after the first keep adding to D)
-template <int K_MAX>
-__device__ __forceinline__ void wg_issue_chunk(uint32_t tmem_base, int d_col, const float* b_hi, const float* b_lo, int n_pad,
-                                               uint32_t accumulate_first, uint64_t* bar) {
-  const uint32_t leader = tc::elect_one();
-  const uint32_t idesc = tc::idesc_tf32(128, n_pad);
-  const uint32_t h32 = ((tc::smem_u32(b_hi) & 0x3ffffu) >> 4) | ((128u >> 4) << 16);
-  const uint32_t l32 = ((tc::smem_u32(b_lo) & 0x3ffffu) >> 4) | ((128u >> 4) << 16);
-  const uint32_t hi32 = (uint32_t)(((kWgTcRows >> 2) * 128) >> 4) | (1u << 14);
-  const uint32_t d = tmem_base + (uint32_t)d_col;
-  for (int ks = 0; ks < kWgTcRows / 8; ++ks) {
-    const uint32_t adv = (uint32_t)(ks * 2 * 128) >> 4;
-    const uint32_t a_hi = tmem_base + (uint32_t)(ks * 8), a_lo = tmem_base + (uint32_t)(K_MAX + ks * 8);
-    const uint64_t dh = ((uint64_t)hi32 << 32) | (h32 + adv), dl = ((uint64_t)hi32 << 32) | (l32 + adv);
-    if (leader) {
-      tc::mma_tf32_ts(d, a_hi, dh, idesc, ks != 0 ? 1u : accumulate_first);
-      tc::mma_tf32_ts(d, a_lo, dh, idesc, 1);
-      tc::mma_tf32_ts(d, a_hi, dl, idesc, 1);
-    }
-  }
-  if (leader) tc::mma_commit(bar);
-  __syncwarp();
-}
 __global__ void __launch_bounds__(128) linear_wgrad_tc_kernel(const float* __restrict__ x, const float* __restrict__ dy, int64_t n_rows,
-                                                              int K, int N, int relu_x, float* __restrict__ dW, float* __restrict__ db,
-                                                              int* __restrict__ status) {
-  using Cols = tc::TileCols<kWgTcRows, 64>;
-  __shared__ __align__(128) float b_tile[2 * 64 * kWgTcRows];  // hi | lo, 24 KB
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(8) uint64_t bar;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int n_pad = (K + 15) / 16 * 16;  // the MMA's N = input width of the layer
-  float* b_hi = b_tile;
-  float* b_lo = b_tile + n_pad * kWgTcRows;
-  if (warp == 0) tc::tmem_alloc(&tmem_base_s, 256);
-  if (tid == 0) tc::mbar_init(&bar, 1);
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, tmem_base_s, 0);
-  const uint32_t lane_base = tmem_base + ((uint32_t)(32 * (warp & 3)) << 16);
-  uint32_t parity = 0, acc = 0;
+                                                              int K, int N, int relu_x, float* __restrict__ dW, float* __restrict__ db) {
+  extern __shared__ __align__(128) float sm[];  // kWgTcSmemBytes
+  const int tid = threadIdx.x;
+  float* b_hi = sm;
+  float* b_lo = sm + kWgTcN * kWgTcRows;
+  float* a_stage = sm + 2 * kWgTcN * kWgTcRows;
+  float acc[kWgTcN];
+#pragma unroll
+  for (int i = 0; i < kWgTcN; ++i) acc[i] = 0.f;
   float bacc = 0.f;
+  bool any = false;
   const int64_t n_chunks = (n_rows + kWgTcRows - 1) / kWgTcRows;
   for (int64_t ch = blockIdx.x; ch < n_chunks; ch += gridDim.x) {
     const int64_t r0 = ch * kWgTcRows;
@@ -618,38 +588,26 @@ __global__ void __launch_bounds__(128) linear_wgrad_tc_kernel(const float* __res
       v[r] = (tid < N && r0 + r < n_rows) ? dy[(r0 + r) * N + tid] : 0.f;
       bacc += v[r];
     }
-    tc::store_a<kWgTcRows>(lane_base, 0, v, kWgTcRows);
-    wg_stage_xt(b_hi, b_lo, x, r0, n_rows, K, n_pad, relu_x != 0, tid, 128);
-    tc::fence_async_smem();
-    tc::wait_st();
-    tc::fence_before_sync();
+    tc::store_row<kWgTcRows>(a_stage, tc::stage_pitch(kWgTcRows), v, kWgTcRows);
+    wg_stage_xt(b_hi, b_lo, x, r0, n_rows, K, kWgTcN, relu_x != 0, tid, 128);
+    tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
     __syncthreads();
-    if (warp == 0) {
-      tc::fence_after_sync();
-      wg_issue_chunk<kWgTcRows>(tmem_base, Cols::d, b_hi, b_lo, n_pad, acc, &bar);
-    }
-    if (!tc::mbar_wait(&bar, parity)) atomicExch(status, 1);  // A (TMEM) and the B tile may be overwritten after this
-    parity ^= 1u;
-    acc = 1u;
-    tc::fence_after_sync();
+    tc::tile_mma<kWgTcN>(a_stage, tc::stage_pitch(kWgTcRows), kWgTcRows, b_hi, b_lo, acc);
+    __syncthreads();  // the A stage and the B tile may be overwritten after this
+    any = true;
   }
-  if (acc) {  // this CTA contributed: drain its accumulator
-    uint32_t d[64];
-    tc::tmem_ld16(lane_base + Cols::d, d);
-    if (n_pad > 16) tc::tmem_ld16(lane_base + Cols::d + 16, d + 16);
-    if (n_pad > 32) tc::tmem_ld16(lane_base + Cols::d + 32, d + 32);
-    if (n_pad > 48) tc::tmem_ld16(lane_base + Cols::d + 48, d + 48);
-    tc::wait_ld();
+  if (any) {  // this CTA contributed: drain its accumulator (uniform across the CTA)
+    tc::tile_store_d<kWgTcN>(sm, kWgTcPitch, acc);
+    __syncthreads();
+    float d[kWgTcN];
+    tc::load_row<kWgTcN>(sm, kWgTcPitch, d, kWgTcN);
     if (tid < N) {
 #pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (i < K) atomicAdd(dW + tid * K + i, __uint_as_float(d[i]));
+      for (int i = 0; i < kWgTcN; ++i)
+        if (i < K) atomicAdd(dW + tid * K + i, d[i]);
       if (db) atomicAdd(db + tid, bacc);
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem_base, 256);
 }
 
 // Gradient of the main field's features with respect to the actor trajectories (DynamicActors.actor_positions /

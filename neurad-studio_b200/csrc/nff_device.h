@@ -229,8 +229,8 @@ NFF_D float trilerp_f(const float f[8], const Cell& c, float ix, float iy, float
 
 // ---- fused-path addressing: byte offsets straight out of the hash --------------------------------------------------
 // The stage operator above exposes the reference's row indices; the fused kernels only need the ADDRESSES, and the
-// index arithmetic was a quarter of their instructions (profiles/r01_ncu_render_v10_split.txt: per corner xor3 + and +
-// zero-extend + 64-bit scale-and-add).  Here every hash term is pre-multiplied by the row size (a shift distributes over
+// index arithmetic was a large share of their instructions (per corner xor3 + and + zero-extend +
+// 64-bit scale-and-add).  Here every hash term is pre-multiplied by the row size (a shift distributes over
 // xor, and (h & mask) << s == (h << s) & (mask << s) while log2(T) + s <= 32), so a corner costs one LOP3
 // ((hx ^ a) & maskb) and one 64-bit add.  The "ceil" corner is always floor + 1: where the reference's ceil equals its
 // floor (p integral) the interpolation offset is exactly 0, so the value read there is multiplied by 0 either way
@@ -512,7 +512,7 @@ template <int ACT_ROWS>
 struct WarpSharedT {
   // The sampling scratch (cdf, resampled bins, euclidean edges) is dead once the main-field phase starts and the
   // activation panel is dead until then, so they share storage: every KB of shared memory given back is L1 cache
-  // for the hash-grid gathers (unified 228 KB L1/shared on sm_100).
+  // for the hash-grid gathers (unified 256 KB L1/shared per SM on sm_90).
   union {
     struct {
       float cdf[kS0 + 4];
@@ -695,7 +695,7 @@ NFF_D void dense(const float* NFF_RESTRICT W, const float* NFF_RESTRICT B, const
 
 // Same product, but the input row lives in the warp's shared-memory panel act[k][lane] and the k-loop stays rolled:
 // keeps the kernel small enough for the instruction cache (the fully unrolled form is ~27k SASS instructions and
-// stalls 40% of the time on instruction fetch, profiles/r01_ncu_render_v1.txt).
+// stalls on instruction fetch).
 template <int IN, int OUT, int OUTP>
 NFF_D void dense_panel(const float* NFF_RESTRICT W, const float* NFF_RESTRICT B, const float (*act)[33], float* acc) {
   const int ln = lane();
@@ -768,7 +768,7 @@ NFF_D float proposal_round(const RenderParams& P, const FieldGrids& fg, WS& ws, 
   syncwarp();
   // NFF_ILP chunks (of 32 samples) are processed together: each lane carries NFF_ILP independent samples through
   // gaussian -> contraction -> gathers -> interpolation, which is what fills the issue slots of a kernel that runs
-  // at 4 warps per scheduler (profiles/r01_ncu_render_v5_tc.txt: stall_wait + long_sb ~ 50 %)
+  // at 4 warps per scheduler
   constexpr int U = NFF_ILP;
 #pragma unroll 1
   for (int s0 = 0; s0 < S; s0 += 32 * U) {
@@ -889,21 +889,22 @@ struct MlpFfma {
 }  // namespace nff
 #include "tc_mlp.cuh"
 namespace nff {
-// Tensor-core path: a tile = the 4 warps (4 rays x 32 samples = 128 rows) of one warp group; activations live in
-// TMEM (columns [A_hi 48 | A_lo 48 | D 32] per tile), weights are tcgen05 B tiles in shared memory, every layer is
-// 3 x (K/8) tcgen05.mma (3xTF32 split, fp32-level accuracy) issued by the group's first thread.  The sdf neuron
-// (row 0 of mlp_geo's last layer) is one 32-term dot product on the CUDA cores so that all tensor-core layers have
-// N = 32 and a tile needs only 128 TMEM columns.
+// Tensor-core path: a tile = the 4 warps (4 rays x 32 samples = 128 rows) of one warp group; every layer is a wgmma
+// tile product through the group's shared-memory stage (tc_mlp.cuh: 3xTF32 split, fp32-level accuracy), the weights are
+// staged once per CTA in shared memory.  The sdf neuron (row 0 of mlp_geo's last layer) is one 32-term dot product on
+// the CUDA cores so that all tensor-core layers have N = 32.
 constexpr int kTcLayers = 5;
-constexpr int kTcTileCols = 128;
+constexpr int kTcPitch = tc::stage_pitch(48);     // stage row pitch (floats) for K <= 48, N = 32
+constexpr int kTcStageFloats = 128 * kTcPitch;    // one warp group's stage (26 KB)
 struct TcShared {
   float b[2 * 32 * (32 + 32 + 48 + 32 + 32)];  // hi|lo B tiles of the 5 layers (45 KB)
   float bias[kTcLayers][32];
   float w_sdf[32];
   float b_sdf;
-  uint32_t tmem_base;
-  uint64_t bar[4];
 };
+constexpr int kTcBytes = (sizeof(TcShared) + 127) / 128 * 128;
+// dynamic shared memory of a tensor-core render kernel up to its own part: TcShared, then one stage per warp group
+constexpr size_t tc_smem_bytes(int threads) { return (size_t)kTcBytes + (size_t)(threads / 128) * kTcStageFloats * sizeof(float); }
 NFF_D constexpr int tc_layer_k(int l) { return l == 2 ? 48 : 32; }
 NFF_D constexpr int tc_layer_off(int l) { return l == 0 ? 0 : l == 1 ? 2048 : l == 2 ? 4096 : l == 3 ? 7168 : 9216; }
 
@@ -924,35 +925,17 @@ NFF_D void tc_stage_weights(TcShared& t, const float* NFF_RESTRICT nn, int tid, 
 
 struct MlpTc {
   const TcShared* t;
-  uint32_t tile_base;  // TMEM address of the tile's first column (lane 0)
-  uint32_t lane_base;  // same, at this warp's lane quarter
-  uint64_t* bar;
-  uint32_t parity;
-  int bar_id;
-  bool issuer;  // warp-uniform: this warp is the first of its 4-warp tile and issues the tile's MMAs
-  int* status;
+  float* stage;  // this warp group's [128][kTcPitch] stage
+  int bar_id;    // this warp group's named barrier
 
-  // store K activations of this thread's row, run layer l on the tensor cores, fetch the 32 outputs
+  // run layer l for this thread's row (K activations) on the tensor cores: the 32 outputs + bias -> out
   template <int K>
   NFF_D void layer(int l, const float* x, float* out) {
-    tc::store_a<48>(lane_base, 0, x, K);
-    tc::wait_st();
-    tc::fence_before_sync();
-    asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-    if (issuer) {
-      tc::fence_after_sync();
-      const float* hi = t->b + tc_layer_off(l);
-      tc::issue_layer<48>(tile_base, 96, hi, hi + 32 * K, K, 32, bar);
-    }
-    if (!tc::mbar_wait(bar, parity) && status) atomicExch(status, 2);
-    parity ^= 1u;
-    tc::fence_after_sync();
-    uint32_t d[32];
-    tc::tmem_ld16(lane_base + 96, d);
-    tc::tmem_ld16(lane_base + 112, d + 16);
-    tc::wait_ld();
+    const float* hi = t->b + tc_layer_off(l);
+    const int id = bar_id;
+    tc::tile_layer<48, 32>(stage, kTcPitch, x, K, hi, hi + 32 * K, out, [id] { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); });
 #pragma unroll
-    for (int i = 0; i < 32; ++i) out[i] = __uint_as_float(d[i]) + t->bias[l][i];
+    for (int i = 0; i < 32; ++i) out[i] += t->bias[l][i];
   }
 
   template <class WS>

@@ -1,6 +1,6 @@
 // nff_lane.h -- "one ray per lane" variant of the fused NFF render.
 //
-// Why: profiling the warp-per-ray kernel (profiles/r01_ncu_render_v5_tc.txt) shows it bound by the L1 tag stage: a
+// Why: profiling the warp-per-ray kernel showed it bound by the L1 tag stage: a
 // gather instruction whose 32 lanes are 32 consecutive samples of ONE ray touches ~13 different 128-byte lines
 // (17 sectors) per request, and neither more loads in flight nor more ILP moved the time.  Here the 32 lanes of a warp
 // are 32 ADJACENT RAYS at the SAME sample index: their positions differ by a pixel footprint, so at the coarse and

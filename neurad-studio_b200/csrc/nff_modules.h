@@ -241,8 +241,8 @@ NFF_D void encode_levels_bwd(float* grad_table, const Grid& gr, const Gauss& g, 
 }
 
 // ---- scatter backward, round 2: registers only + run-length aggregation of the coarse levels ---------------------------
-// What bounds the scatter (profiles/r02_ncu_encoding_bwd.txt): not instructions and not DRAM but the L2 atomic units of a
-// FEW slices -- lts__t_tag_requests is 80 % of peak on the busiest slice and 25 % on average.  Every ray starts at the
+// What bounds the scatter: not instructions and not DRAM but the L2 atomic units of a FEW slices (the busiest
+// slice's tag requests run far above the average).  Every ray starts at the
 // sensor, so the coarse levels' cells around the sensors receive a reduction from every near-range sample of every ray,
 // and same-address reductions serialise in the slice that owns the row.  Consecutive samples of a ray share their coarse
 // cells, so a thread that walks a CONTIGUOUS segment of one ray keeps the current cell's 8 corner sums of the first K

@@ -3,8 +3,9 @@
 //   -> Conv2d(32->3, 1x1) -> Sigmoid,            feature image [B,H,W,in] (row-major rays) -> rgb [B,3H,3W,3].
 //
 // 97 % of the work is the eight 7x7 convolutions (50 176 MAC per pixel each).  They run as implicit GEMMs on the
-// tcgen05 tensor cores: M = 128 consecutive pixels of one image row, N = 32 output channels, K = 49 taps x 32 input
-// channels, fp32 accumulators in TMEM.  BatchNorm is folded into the conv weights/bias when the parameters are set.
+// Hopper warp-group tensor cores (wgmma): M = 128 consecutive pixels of one image row (two m64 tiles, one per warp
+// group), N = 32 output channels, K = 49 taps x 32 input channels, fp32 accumulators in registers.  BatchNorm is folded
+// into the conv weights/bias when the parameters are set.
 //
 // fp32-level accuracy from bf16 tensor-core inputs: every activation and weight is split into two bf16 numbers
 // (hi = bf16(v), lo = bf16(v - hi)) and each k-step issues three MMAs  a_hi*w_hi + a_lo*w_hi + a_hi*w_lo  into the
@@ -14,23 +15,22 @@
 // Activations between layers therefore live in HBM already split ("ACT" layout): per pixel 128 B = 8 chunks of 8 bf16,
 // chunk c < 4: hi of channels 8c..8c+7, chunk 4+c: lo.  A conv CTA copies a (4+6) x (128+6) pixel window of it into
 // shared memory as 8 planes [chunk][row][pixel][16 B]; in that layout the A operand of tap (dy,dx) for output row r is
-// the SAME planes read from a shifted start address ((r+dy)*PW + dx)*16 B -- the canonical K-major no-swizzle UMMA
+// the SAME planes read from a shifted start address ((r+dy)*PW + dx)*16 B -- the canonical K-major no-swizzle GMMA
 // layout with SBO = 128 B (8-pixel groups are contiguous) and LBO = the plane stride -- so the im2col matrix is never
 // materialised.  The folded weights of one tap COLUMN dx ({hi,lo} x 7 taps x 32x32 bf16 = 28 KB, pre-arranged in the
-// UMMA B layout by dec_fold_conv_kernel) are double-buffered in shared memory and streamed from L2 while the tensor
+// GMMA B layout by dec_fold_conv_kernel) are double-buffered in shared memory and streamed from L2 while the tensor
 // core works on the previous column.
 //
-// Shared-memory bandwidth, not the tensor pipe, bounds an SS-mode MMA this narrow (128 x 32 x 16: 4 KB of A per 65 k
-// MAC), so the loop is arranged to read each A block once for ALL the output rows it feeds: input row i at shift dx
-// contributes to output row r through tap dy = i - r, for up to four r at once.  With the four accumulators side by
-// side in TMEM ([D0|D1|D2|D3], 32 columns each) and the tap tiles stored in descending dy, that is ONE MMA with N = 128
-// (N = 32..96 at the window's top and bottom rows): 420 MMAs per 4-row tile instead of 1176.  Measured, the operand
-// fetch sustains ~64 B/clk, which makes shared-memory bytes per MAC the bound of this kernel (profiles/).  The accumulators start from the folded bias (written with tcgen05.st), every MMA accumulates.
+// Each A block is read once for ALL the output rows it feeds: input row i at shift dx feeds output row r through tap
+// dy = i - r.  With the four accumulators side by side ([D0|D1|D2|D3]) and the tap tiles in descending dy, that is ONE
+// MMA with N = 32..128.  The accumulators start from the folded bias.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <utility>
 
 #include "tc_mlp.cuh"
 
@@ -48,9 +48,7 @@ constexpr int kPlaneBytes = (kIR * kPW * 16 + 127) / 128 * 128;  // TMA destinat
 constexpr int kActBytes = 8 * kPlaneBytes;
 constexpr int kWTileBytes = kC * kC * 2;                 // one 32x32 bf16 B tile
 constexpr int kWRowBytes = kK7 * 2 * kWTileBytes;        // one tap column: {hi, lo} x 7 taps (dy descending)
-constexpr int kConvThreads = 256;
-constexpr int kTmemCols = 128;                           // kTH accumulators x 32 columns, power of two
-static_assert(kTH * kC <= kTmemCols, "accumulators do not fit the TMEM allocation");
+constexpr int kConvThreads = 256;                        // two warp groups, 64 pixels of the strip each
 
 struct ConvSmem {
   alignas(128) unsigned char act[kActBytes];
@@ -58,12 +56,9 @@ struct ConvSmem {
   float bias[kC];
   float out_w[3 * kC];
   float out_b[4];
-  alignas(8) uint64_t bar[2];      // MMA completion per weight buffer
   alignas(8) uint64_t bar_w[2];    // TMA kernel: weight column landed in w[b]
   alignas(8) uint64_t bar_win;     // TMA kernel: input window landed
-  alignas(8) uint64_t bar_done;    // TMA kernel: every MMA of the tile has completed (one commit per tile)
-  uint32_t tmem_base;
-  volatile int abort;  // a completion barrier timed out: every thread leaves at the next block-wide sync
+  volatile int abort;  // a completion barrier timed out: every thread leaves after the tile's last block-wide sync
 };
 
 static_assert(sizeof(ConvSmem) <= 227 * 1024, "ConvSmem exceeds the 227 KB a CTA may opt in to");
@@ -111,9 +106,9 @@ __device__ __forceinline__ void load_act(const uint4* src, float* v) {
 // ---------------------------------------------------------------------------------------- parameter preparation
 // Conv2d [co][ci][7][7] + BatchNorm2d (eval) -> folded  w' = w * s[co],  b' = (b - mean) * s + beta,  s = gamma /
 // sqrt(var + eps)  (BasicBlock.main_branch, cnns.py:37-43), written as
-//   w_img : [dx][hi|lo][6 - dy] 32x32 bf16 tiles in the UMMA K-major no-swizzle B layout (n = co, k = ci):
+//   w_img : [dx][hi|lo][6 - dy] 32x32 bf16 tiles in the GMMA K-major no-swizzle B layout (n = co, k = ci):
 //           byte offset of (n,k) = (n/8)*512 + (k/8)*128 + (n%8)*16 + (k%8)*2.  Tiles of one tap COLUMN are contiguous
-//           in DESCENDING dy, so that [W(dy), W(dy-1), W(dy-2)] is one N = 96 B operand (see dec_conv7_tc_kernel)
+//           in DESCENDING dy, so that [W(dy), W(dy-1), W(dy-2)] is one N = 96 B operand (see issue_window_row)
 //   w_f32 : [dy][dx][ci][co] fp32 (CUDA-core reference kernel)
 //   bias  : [co]
 __global__ void dec_fold_conv_kernel(const float* __restrict__ w, const float* __restrict__ b, const float* __restrict__ gamma,
@@ -242,70 +237,6 @@ __device__ __forceinline__ void conv_epilogue(float* acc, const uint4* __restric
   }
 }
 
-// ------------------------------------------------------------------------------- 7x7 conv on the tensor cores
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version 1 [46,48), SWIZZLE_NONE
-  return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-// cute::UMMA::InstrDescriptor for kind::f16: D = F32 (1<<4), A = B = BF16 (1<<7, 1<<10), both K-major, N>>3, M>>4
-__host__ __device__ constexpr uint32_t idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void mma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Bounded completion wait (a wrong descriptor must surface as a failed status, not as a wedged GPU).
-__device__ __forceinline__ bool bar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = tc::smem_u32(bar);
-  for (int it = 0; it < (1 << 17); ++it) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (ok) return true;
-  }
-  return false;
-}
-
-__device__ __forceinline__ uint32_t elect_one() {  // one lane of the converged warp (the same one every time)
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred;
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-
-// 16-byte asynchronous global -> shared copy (LDGSTS); src_bytes = 0 writes zeros (the conv's padding) without
-// reading.  Many of these are in flight per thread, which is what hides the L2 latency of the window / weight loads.
-__device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
-// this thread's TMEM lane, 32 accumulator columns <- the folded bias
-__device__ __forceinline__ void arm_accumulator(uint32_t taddr, const float* bias) {
-#pragma unroll
-  for (int c = 0; c < kC; c += 8) {
-    uint32_t v[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = __float_as_uint(bias[c + k]);
-    tc::tmem_st8(taddr + (uint32_t)c, v);
-  }
-}
-
 struct ConvArgs {
   const uint4* in;        // ACT [B][H][W]
   const uint4* residual;  // ACT (EPI_RES_*) or nullptr
@@ -320,166 +251,107 @@ struct ConvArgs {
   int* status;
 };
 
-template <int EPI>
-__global__ void __launch_bounds__(kConvThreads, 1) dec_conv7_tc_kernel(const ConvArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  ConvSmem& S = *reinterpret_cast<ConvSmem*>(smem_raw);
-  const int tid = threadIdx.x, ln = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform
-  if (tid < kC) S.bias[tid] = a.bias[tid];
-  if (EPI == EPI_RES_RELU_RGB) {
-    if (tid < 3 * kC) S.out_w[tid] = a.out_w[tid];
-    if (tid < 3) S.out_b[tid] = a.out_b[tid];
-  }
-  if (warp == 0) tc::tmem_alloc(&S.tmem_base, kTmemCols);
-  if (tid == 0) {
-    tc::mbar_init(&S.bar[0], 1);
-    tc::mbar_init(&S.bar[1], 1);
-    S.abort = 0;
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, S.tmem_base, 0);
-  // low 32 bits of the shared-memory descriptors: start address >> 4 in [0,14), LBO >> 4 in [16,30); the high words
-  // (SBO >> 4, version 1, no swizzle) are constants.  Advancing an operand = adding 16-byte units to the low word.
-  const uint32_t a_lo32 = ((tc::smem_u32(S.act) & 0x3ffffu) >> 4) | ((uint32_t)(kPlaneBytes >> 4) << 16);
-  const uint32_t b_lo32[2] = {((tc::smem_u32(S.w[0]) & 0x3ffffu) >> 4) | ((128u >> 4) << 16),
-                              ((tc::smem_u32(S.w[1]) & 0x3ffffu) >> 4) | ((128u >> 4) << 16)};
-  const uint32_t act_u32 = tc::smem_u32(S.act);
-  const uint32_t w_u32[2] = {tc::smem_u32(S.w[0]), tc::smem_u32(S.w[1])};
-  constexpr uint32_t kDescHiA = (128u >> 4) | (1u << 14), kDescHiB = (512u >> 4) | (1u << 14);  // bits [32,64)
-  uint32_t parity[2] = {0u, 0u};
+// ------------------------------------------------------------------------------- 7x7 conv on the tensor cores
+// Both operands K-major, no swizzle.  A: LBO = plane stride, SBO = 128 B (8 pixels).  B: LBO = 128 B, SBO = 512 B.
+constexpr uint32_t kDescSboA = 128u, kDescLboB = 128u, kDescSboB = 512u;
 
-  const int tiles_x = (a.W + kStrip - 1) / kStrip, tiles_y = (a.H + kTH - 1) / kTH;
-  const int64_t n_tiles = (int64_t)a.batch * tiles_y * tiles_x;
-  // asynchronous fill of the input window (8 chunk planes; pixels outside the image are the conv's zero padding) and of
-  // tap row 0 of the weights for one tile
-  auto issue_tile_loads = [&](int64_t tile) {
-    const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y);
-    const int64_t img = tile / ((int64_t)tiles_x * tiles_y);
-    const int x0 = tx * kStrip, y0 = ty * kTH;
-    const uint4* in_img = a.in + img * (int64_t)a.H * a.W * 8;
-    for (int i = tid; i < kIR * kPW * 8; i += kConvThreads) {
-      const int c = i & 7, ip = (i >> 3) % kPW, ir = (i >> 3) / kPW;
-      const int y = y0 - kPad + ir, x = x0 - kPad + ip;
-      const bool inside = y >= 0 && y < a.H && x >= 0 && x < a.W;
-      const uint4* src = inside ? in_img + ((int64_t)y * a.W + x) * 8 + c : in_img;
-      cp_async16(act_u32 + (uint32_t)(c * kPlaneBytes + (ir * kPW + ip) * 16), src, inside ? 16u : 0u);
-    }
-    const uint4* src = reinterpret_cast<const uint4*>(a.w_img);
-    for (int i = tid; i < kWRowBytes / 16; i += kConvThreads) cp_async16(w_u32[0] + (uint32_t)(i * 16), src + i, 16u);
-  };
-  if ((int64_t)blockIdx.x < n_tiles) issue_tile_loads(blockIdx.x);
-  for (int r = warp >> 2; r < kTH; r += 2) arm_accumulator(tmem + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(r * kC), S.bias);
-  tc::wait_st();
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y);
-    const int64_t img = tile / ((int64_t)tiles_x * tiles_y);
-    const int x0 = tx * kStrip, y0 = ty * kTH;
-    cp_async_wait_all();
-    tc::fence_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
-    tc::fence_before_sync();
-    __syncthreads();
-    for (int dx = 0; dx < kK7; ++dx) {
-      const int buf = dx & 1, nb = buf ^ 1;
-      if (warp == 0) {
-        // The whole (converged) warp walks the loop so that every descriptor is a warp-uniform value the compiler keeps
-        // in uniform registers -- tcgen05.mma takes its operands from there; built inside a single-thread branch each
-        // MMA pays a register->uniform broadcast loop -- and one elected lane issues.
-        tc::fence_after_sync();
-        const uint32_t leader = elect_one();
-#pragma unroll
-        for (int i = 0; i < kIR; ++i) {  // input row i feeds output rows r_min..r_max through taps dy = i - r
-          constexpr int kLast = kK7 - 1;
-          const int r_min = i > kLast ? i - kLast : 0, r_max = i < kTH - 1 ? i : kTH - 1, nr = r_max - r_min + 1;
-          const uint32_t d = tmem + (uint32_t)(r_min * kC);
-          const uint32_t idesc = idesc_bf16(kStrip, kC * nr);
-          const uint32_t slot = (uint32_t)(kLast - (i - r_min));  // first (largest-dy) tile of the N-concatenated B
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {  // 16 input channels (two 8-channel chunks) per MMA
-            const uint32_t ah = a_lo32 + (uint32_t)(i * kPW + 2 * ks * (kPlaneBytes / 16)) + (uint32_t)dx;
-            const uint32_t al = ah + (uint32_t)(4 * (kPlaneBytes / 16));
-            const uint32_t bh = b_lo32[buf] + (slot * kWTileBytes + (uint32_t)(ks * 256)) / 16;
-            const uint32_t bl = bh + (uint32_t)(kK7 * kWTileBytes / 16);
-            if (leader) {
-              mma_bf16_ss(d, make_desc(ah, kDescHiA), make_desc(bh, kDescHiB), idesc, 1);
-              mma_bf16_ss(d, make_desc(al, kDescHiA), make_desc(bh, kDescHiB), idesc, 1);
-              mma_bf16_ss(d, make_desc(ah, kDescHiA), make_desc(bl, kDescHiB), idesc, 1);
-            }
-          }
-        }
-        if (leader) tc::mma_commit(&S.bar[buf]);
-        __syncwarp();
-        if (dx >= 1 && dx + 1 < kK7) parity[nb] ^= 1u;  // keep the phase bookkeeping of the loading warps
-      } else if (dx + 1 < kK7) {
-        // warps 1..7 stream the next tap column while warp 0 is busy issuing
-        if (dx >= 1) {  // the MMAs of column dx-1 read w[nb]: wait for them before overwriting it
-          if (!bar_wait(&S.bar[nb], parity[nb])) S.abort = 1;
-          parity[nb] ^= 1u;
-        }
-        const uint4* src = reinterpret_cast<const uint4*>(a.w_img + (size_t)(dx + 1) * kWRowBytes);
-        for (int i = tid - 32; i < kWRowBytes / 16; i += kConvThreads - 32) cp_async16(w_u32[nb] + (uint32_t)(i * 16), src + i, 16u);
-        cp_async_wait_all();
-        tc::fence_async_smem();
-      }
-      if (dx + 1 < kK7) {
-        tc::fence_before_sync();
-        __syncthreads();
-        if (S.abort) break;
-      }
-    }
-    if (S.abort) break;
-    // tap columns 5 (bar[1]) and 6 (bar[0]) are still outstanding; the commit of column 6 covers every earlier MMA
-    if (!bar_wait(&S.bar[1], parity[1])) S.abort = 1;
-    parity[1] ^= 1u;
-    if (!bar_wait(&S.bar[0], parity[0])) S.abort = 1;
-    parity[0] ^= 1u;
-    tc::fence_after_sync();
-    // every MMA of this tile has completed: the window and both weight buffers are free, so the next tile's loads fly
-    // while this tile's accumulators are drained
-    if (tile + gridDim.x < n_tiles) issue_tile_loads(tile + gridDim.x);
-    // ---- epilogue: warps 0-3 take output rows 0 and 2, warps 4-7 rows 1 and 3; a thread owns one pixel (= TMEM lane)
-    const uint32_t lane_base = tmem + ((uint32_t)(32 * (warp & 3)) << 16);
-    const int m = 32 * (warp & 3) + ln;
-    for (int r = warp >> 2; r < kTH; r += 2) {
-      uint32_t dreg[kC];
-      tc::tmem_ld16(lane_base + (uint32_t)(r * kC), dreg);
-      tc::tmem_ld16(lane_base + (uint32_t)(r * kC + 16), dreg + 16);
-      tc::wait_ld();
-      arm_accumulator(lane_base + (uint32_t)(r * kC), S.bias);  // folded bias: the next tile's MMAs all accumulate
-      const int y = y0 + r, x = x0 + m;
-      if (y < a.H && x < a.W) {
-        float acc[kC];
-#pragma unroll
-        for (int k = 0; k < kC; ++k) acc[k] = __uint_as_float(dreg[k]);
-        const int64_t pix = (img * a.H + y) * a.W + x;
-        conv_epilogue<EPI>(acc, a.residual, pix, a.out_act, a.out_rgb, S.out_w, S.out_b);
-      }
-    }
-    tc::wait_st();
-    tc::fence_before_sync();
-    __syncthreads();  // accumulators and the input window are free again
-    tc::fence_after_sync();
-    if (S.abort) break;
-  }
-  cp_async_wait_all();
-  if (S.abort && tid == 0 && a.status) atomicExch(a.status, 2);
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem, kTmemCols);
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t a_desc, uint64_t b_desc) {
+  static_assert(N == 32 || N == 64 || N == 96 || N == 128, "one to four 32-channel accumulators");
+  if constexpr (N == 32) tc::wgmma_bf16_m64n32(d, a_desc, b_desc);
+  else if constexpr (N == 64) tc::wgmma_bf16_m64n64(d, a_desc, b_desc);
+  else if constexpr (N == 96) tc::wgmma_bf16_m64n96(d, a_desc, b_desc);
+  else tc::wgmma_bf16_m64n128(d, a_desc, b_desc);
 }
 
-// ---------------------------------------------------------------- 7x7 conv on the tensor cores, TMA operand loads
-// Same tile loop and MMA schedule as dec_conv7_tc_kernel, but the operands are moved by the TMA engine instead of
-// 16-byte LDGSTS issued by every thread (9 648 per tile: the LSU issue alone cost ~11 k cycles per tile):
-//   * the input window is 8 tensor copies (one per chunk plane) from a 5-D tensor map over the ACT buffer
-//     [image][y][x][chunk][8 bf16] with box (8, 1, 134, 9, 1); coordinates may be negative / beyond the image, the TMA
-//     zero-fills, which IS the convolution's padding;
-//   * a weight column is one 28 KB bulk copy.
-// One elected lane of warp 1 is the producer, warp 0 issues the MMAs; they hand buffers to each other through mbarriers
-// (transaction-count barriers for the loads, tcgen05.commit barriers for the MMAs), so the tap-column loop has no
-// block-wide barrier at all.  All 8 warps run the epilogue.
+// Input row I of the window at tap column dx feeds output rows r_min..r_max through taps dy = I - r: one wgmma per
+// operand pair with N = 32 * (rows fed), accumulating into those rows' registers (acc + 16 * r_min).
+template <int I>
+__device__ __forceinline__ void issue_window_row(float* acc, uint32_t a_row, uint32_t w_buf) {
+  constexpr int kLast = kK7 - 1;
+  constexpr int r_min = I > kLast ? I - kLast : 0, r_max = I < kTH - 1 ? I : kTH - 1, nr = r_max - r_min + 1;
+  constexpr uint32_t slot = (uint32_t)(kLast - (I - r_min));  // first (largest-dy) tile of the N-concatenated B
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) {  // 16 input channels (two 8-channel chunks) per MMA
+    const uint32_t ah = a_row + (uint32_t)(I * kPW * 16 + 2 * ks * kPlaneBytes);
+    const uint32_t al = ah + (uint32_t)(4 * kPlaneBytes);
+    const uint32_t bh = w_buf + slot * kWTileBytes + (uint32_t)(ks * 256);
+    const uint32_t bl = bh + (uint32_t)(kK7 * kWTileBytes);
+    const uint64_t dah = tc::smem_desc(ah, kPlaneBytes, kDescSboA), dal = tc::smem_desc(al, kPlaneBytes, kDescSboA);
+    const uint64_t dbh = tc::smem_desc(bh, kDescLboB, kDescSboB), dbl = tc::smem_desc(bl, kDescLboB, kDescSboB);
+    wgmma_bf16<32 * nr>(acc + 16 * r_min, dah, dbh);
+    wgmma_bf16<32 * nr>(acc + 16 * r_min, dal, dbh);
+    wgmma_bf16<32 * nr>(acc + 16 * r_min, dah, dbl);
+  }
+}
+template <int... I>
+__device__ __forceinline__ void issue_window_rows(float* acc, uint32_t a_row, uint32_t w_buf, std::integer_sequence<int, I...>) {
+  (issue_window_row<I>(acc, a_row, w_buf), ...);
+}
+
+// Epilogue on the fragments of one output row (pixels lane/4 and lane/4 + 8 of the warp's 16, channels 8j + 2*(lane%4)
+// + {0,1}): 32-bit ACT words per thread; the rgb head reduces its dot products over the 4 lanes of a pixel.
+template <int EPI>
+__device__ __forceinline__ void conv_epilogue_frag(const float* d, const ConvArgs& a, int64_t pix0, bool ok0, int64_t pix1, bool ok1,
+                                                   int t, const float* out_w, const float* out_b) {
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const int64_t pix = q ? pix1 : pix0;
+    const bool ok = q ? ok1 : ok0;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      v[2 * j] = d[4 * j + 2 * q];
+      v[2 * j + 1] = d[4 * j + 2 * q + 1];
+    }
+    if (EPI != EPI_RELU && ok) {
+      const uint32_t* res = reinterpret_cast<const uint32_t*>(a.residual + pix * 8);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float x0, x1;
+        unpack2(res[4 * j + t], res[4 * (4 + j) + t], x0, x1);
+        v[2 * j] += x0;
+        v[2 * j + 1] += x1;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.f);
+    if (EPI == EPI_RES_RELU_RGB) {
+      float s[3];
+#pragma unroll
+      for (int o = 0; o < 3; ++o) {
+        s[o] = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          s[o] = fmaf(v[2 * j], out_w[o * kC + 8 * j + 2 * t], s[o]);
+          s[o] = fmaf(v[2 * j + 1], out_w[o * kC + 8 * j + 2 * t + 1], s[o]);
+        }
+        s[o] += __shfl_xor_sync(0xffffffffu, s[o], 1);
+        s[o] += __shfl_xor_sync(0xffffffffu, s[o], 2);
+      }
+      if (ok && t < 3) a.out_rgb[pix * 3 + t] = 1.0f / (1.0f + expf(-(out_b[t] + s[t])));
+    } else if (ok) {
+      uint32_t* dst = reinterpret_cast<uint32_t*>(a.out_act + pix * 8);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        uint32_t h, l;
+        split_pack2(v[2 * j], v[2 * j + 1], h, l);
+        dst[4 * j + t] = h;
+        dst[4 * (4 + j) + t] = l;
+      }
+    }
+  }
+}
+
+// 16-byte asynchronous global -> shared copy (LDGSTS); src_bytes = 0 writes zeros (the conv's padding) without
+// reading.  Many of these are in flight per thread, which is what hides the L2 latency of the window / weight loads.
+__device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc::smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -500,161 +372,136 @@ struct ConvArgsTma {
   ConvArgs a;
 };
 
-template <int EPI>
-__global__ void __launch_bounds__(kConvThreads, 1) dec_conv7_tma_kernel(const __grid_constant__ ConvArgsTma P) {
+// Two warp groups split the 128-pixel strip, each holding the accumulators of all 4 output rows of its 64 pixels.  TMA:
+// the window is 8 tensor copies from a 5-D map over the ACT buffer (its zero fill IS the conv's padding), a weight column
+// one 28 KB bulk copy, issued by thread 0 on transaction-count mbarriers.  Otherwise every thread issues 16-byte LDGSTS.
+// Column dx + 2 is loaded into the buffer column dx has just finished with; the next tile's loads overlap the epilogue.
+template <int EPI, bool TMA>
+__device__ __forceinline__ void conv7_body(const ConvArgs& a, const CUtensorMap* in_map) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   ConvSmem& S = *reinterpret_cast<ConvSmem*>(smem_raw);
-  const ConvArgs& a = P.a;
-  const int tid = threadIdx.x, ln = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform
+  const int tid = threadIdx.x, wgp = tid >> 7, wq = (tid >> 5) & 3, ln = tid & 31, g = ln >> 2, t = ln & 3;
   if (tid < kC) S.bias[tid] = a.bias[tid];
   if (EPI == EPI_RES_RELU_RGB) {
     if (tid < 3 * kC) S.out_w[tid] = a.out_w[tid];
     if (tid < 3) S.out_b[tid] = a.out_b[tid];
   }
-  if (warp == 0) tc::tmem_alloc(&S.tmem_base, kTmemCols);
   if (tid == 0) {
-    tc::mbar_init(&S.bar[0], 1);
-    tc::mbar_init(&S.bar[1], 1);
     tc::mbar_init(&S.bar_w[0], 1);
     tc::mbar_init(&S.bar_w[1], 1);
     tc::mbar_init(&S.bar_win, 1);
-    tc::mbar_init(&S.bar_done, 1);
     S.abort = 0;
   }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, S.tmem_base, 0);
-  const uint32_t a_lo32 = ((tc::smem_u32(S.act) & 0x3ffffu) >> 4) | ((uint32_t)(kPlaneBytes >> 4) << 16);
-  const uint32_t b_lo32[2] = {((tc::smem_u32(S.w[0]) & 0x3ffffu) >> 4) | ((128u >> 4) << 16),
-                              ((tc::smem_u32(S.w[1]) & 0x3ffffu) >> 4) | ((128u >> 4) << 16)};
   const uint32_t act_u32 = tc::smem_u32(S.act);
   const uint32_t w_u32[2] = {tc::smem_u32(S.w[0]), tc::smem_u32(S.w[1])};
-  constexpr uint32_t kDescHiA = (128u >> 4) | (1u << 14), kDescHiB = (512u >> 4) | (1u << 14);  // bits [32,64)
-  constexpr uint32_t kWinBytes = 8u * kIR * kPW * 16u;
-
   const int tiles_x = (a.W + kStrip - 1) / kStrip, tiles_y = (a.H + kTH - 1) / kTH;
   const int64_t n_tiles = (int64_t)a.batch * tiles_y * tiles_x;
-  // per-barrier completion counters (identical in every thread): phase parity of completion #k is k & 1
-  uint32_t n_mma[2] = {0u, 0u}, n_w[2] = {0u, 0u}, n_win = 0u;
-  const bool producer_warp = warp == 1;
+  uint32_t n_w[2] = {0u, 0u}, n_win = 0u;  // TMA: completions waited for so far (phase parity = count & 1)
 
-  // producer: window of `tile` -> act planes, tap column 0 -> w[0]
-  auto issue_tile_loads = [&](int64_t tile) {
+  auto load_window = [&](int64_t tile) {  // TMA: thread 0 only; LDGSTS: every thread, no commit (joins column 0's group)
     const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y);
-    const int img = (int)(tile / ((int64_t)tiles_x * tiles_y));
-    mbar_expect_tx(&S.bar_win, kWinBytes);
+    const int64_t img = tile / ((int64_t)tiles_x * tiles_y);
+    if constexpr (TMA) {
+      constexpr uint32_t kWinBytes = 8u * kIR * kPW * 16u;
+      mbar_expect_tx(&S.bar_win, kWinBytes);
 #pragma unroll
-    for (int c = 0; c < 8; ++c)
-      tma_load_5d(act_u32 + (uint32_t)(c * kPlaneBytes), &P.in_map, 0, c, tx * kStrip - kPad, ty * kTH - kPad, img, &S.bar_win);
-    mbar_expect_tx(&S.bar_w[0], kWRowBytes);
-    bulk_load(w_u32[0], a.w_img, kWRowBytes, &S.bar_w[0]);
+      for (int c = 0; c < 8; ++c)
+        tma_load_5d(act_u32 + (uint32_t)(c * kPlaneBytes), in_map, 0, c, tx * kStrip - kPad, ty * kTH - kPad, (int)img, &S.bar_win);
+    } else {
+      const int x0 = tx * kStrip, y0 = ty * kTH;
+      const uint4* in_img = a.in + img * (int64_t)a.H * a.W * 8;
+      for (int i = tid; i < kIR * kPW * 8; i += kConvThreads) {
+        const int c = i & 7, ip = (i >> 3) % kPW, ir = (i >> 3) / kPW;
+        const int y = y0 - kPad + ir, x = x0 - kPad + ip;
+        const bool inside = y >= 0 && y < a.H && x >= 0 && x < a.W;
+        const uint4* src = inside ? in_img + ((int64_t)y * a.W + x) * 8 + c : in_img;
+        cp_async16(act_u32 + (uint32_t)(c * kPlaneBytes + (ir * kPW + ip) * 16), src, inside ? 16u : 0u);
+      }
+    }
   };
-  if (producer_warp && (int64_t)blockIdx.x < n_tiles) {
-    if (elect_one()) issue_tile_loads(blockIdx.x);
-    __syncwarp();
-  }
-  for (int r = warp >> 2; r < kTH; r += 2) arm_accumulator(tmem + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(r * kC), S.bias);
-  tc::wait_st();
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
+  auto load_column = [&](int dx, int buf) {
+    if constexpr (TMA) {
+      mbar_expect_tx(&S.bar_w[buf], kWRowBytes);
+      bulk_load(w_u32[buf], a.w_img + (size_t)dx * kWRowBytes, kWRowBytes, &S.bar_w[buf]);
+    } else {
+      const uint4* src = reinterpret_cast<const uint4*>(a.w_img + (size_t)dx * kWRowBytes);
+      for (int i = tid; i < kWRowBytes / 16; i += kConvThreads) cp_async16(w_u32[buf] + (uint32_t)(i * 16), src + i, 16u);
+      cp_async_commit();
+    }
+  };
+  auto load_tile_start = [&](int64_t tile) {
+    if (!TMA || tid == 0) {
+      load_window(tile);
+      load_column(0, 0);
+      load_column(1, 1);
+    }
+  };
+  if ((int64_t)blockIdx.x < n_tiles) load_tile_start(blockIdx.x);
 
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y);
     const int64_t img = tile / ((int64_t)tiles_x * tiles_y);
     const int x0 = tx * kStrip, y0 = ty * kTH;
-    if (warp == 0) {
-      // ---- MMA warp: window landed, then per tap column: column landed -> 54 MMAs -> commit
-      if (!bar_wait(&S.bar_win, n_win & 1u)) S.abort = 1;
-      tc::fence_after_sync();
-      const uint32_t leader = elect_one();
+    // accumulators start from the folded bias: row r in acc[16r, 16r + 16), fragment layout of an m64n32 tile
+    float acc[kTH * 16];
+#pragma unroll
+    for (int r = 0; r < kTH; ++r)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        acc[16 * r + 4 * j + 0] = acc[16 * r + 4 * j + 2] = S.bias[8 * j + 2 * t];
+        acc[16 * r + 4 * j + 1] = acc[16 * r + 4 * j + 3] = S.bias[8 * j + 2 * t + 1];
+      }
+    if constexpr (TMA) {
+      if (!tc::mbar_wait(&S.bar_win, n_win & 1u)) S.abort = 1;
+      ++n_win;
+    }
+    const uint32_t a_row = act_u32 + (uint32_t)(64 * wgp * 16);  // this warp group's first pixel in window row 0
 #pragma unroll 1
-      for (int dx = 0; dx < kK7; ++dx) {
-        const int buf = dx & 1;
-        if (!bar_wait(&S.bar_w[buf], (n_w[buf] + (uint32_t)(dx >> 1)) & 1u)) S.abort = 1;
-        tc::fence_after_sync();
-#pragma unroll
-        for (int i = 0; i < kIR; ++i) {  // input row i feeds output rows r_min..r_max through taps dy = i - r
-          constexpr int kLast = kK7 - 1;
-          const int r_min = i > kLast ? i - kLast : 0, r_max = i < kTH - 1 ? i : kTH - 1, nr = r_max - r_min + 1;
-          const uint32_t d = tmem + (uint32_t)(r_min * kC);
-          const uint32_t idesc = idesc_bf16(kStrip, kC * nr);
-          const uint32_t slot = (uint32_t)(kLast - (i - r_min));
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            const uint32_t ah = a_lo32 + (uint32_t)(i * kPW + 2 * ks * (kPlaneBytes / 16)) + (uint32_t)dx;
-            const uint32_t al = ah + (uint32_t)(4 * (kPlaneBytes / 16));
-            const uint32_t bh = b_lo32[buf] + (slot * kWTileBytes + (uint32_t)(ks * 256)) / 16;
-            const uint32_t bl = bh + (uint32_t)(kK7 * kWTileBytes / 16);
-            if (leader) {
-              mma_bf16_ss(d, make_desc(ah, kDescHiA), make_desc(bh, kDescHiB), idesc, 1);
-              mma_bf16_ss(d, make_desc(al, kDescHiA), make_desc(bh, kDescHiB), idesc, 1);
-              mma_bf16_ss(d, make_desc(ah, kDescHiA), make_desc(bl, kDescHiB), idesc, 1);
-            }
-          }
-        }
-        if (leader) tc::mma_commit(&S.bar[buf]);
-        __syncwarp();
+    for (int dx = 0; dx < kK7; ++dx) {
+      const int buf = dx & 1;
+      if constexpr (TMA) {
+        if (!tc::mbar_wait(&S.bar_w[buf], n_w[buf] & 1u)) S.abort = 1;
+        ++n_w[buf];
+      } else {
+        if (dx + 1 < kK7) cp_async_wait<1>(); else cp_async_wait<0>();  // column dx (and the window) have landed
+        tc::fence_async_smem();  // generic-proxy writes -> visible to the tensor cores (async proxy)
+        __syncthreads();
       }
-      if (leader) tc::mma_commit(&S.bar_done);
-      __syncwarp();
-    } else if (producer_warp) {
-      // ---- producer: column dx+1 into the buffer the MMAs of column dx-1 have finished reading
-      const uint32_t leader = elect_one();
-#pragma unroll 1
-      for (int dx = 0; dx + 1 < kK7; ++dx) {
-        const int nb = (dx & 1) ^ 1;
-        if (dx >= 1 && !bar_wait(&S.bar[nb], (n_mma[nb] + (uint32_t)((dx - 1) >> 1)) & 1u)) S.abort = 1;
-        if (leader) {
-          mbar_expect_tx(&S.bar_w[nb], kWRowBytes);
-          bulk_load(w_u32[nb], a.w_img + (size_t)(dx + 1) * kWRowBytes, kWRowBytes, &S.bar_w[nb]);
-        }
-        __syncwarp();
-      }
+      const uint32_t a_dx = a_row + (uint32_t)(dx * 16);
+      tc::wg_fence();
+      issue_window_rows(acc, a_dx, w_u32[buf], std::make_integer_sequence<int, kIR>{});
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      __syncthreads();  // both warp groups are done with w[buf] (after column 6: with the window too)
+      if (dx + 2 < kK7 && (!TMA || tid == 0)) load_column(dx + 2, buf);
     }
-    // Every warp waits for the tile's ONE bar_done completion.  (A parity wait is only sound for a waiter that is at
-    // most one completion behind or ahead of the barrier, so the epilogue warps, which skip the per-column
-    // completions, get their own once-per-tile barrier; the producer and the MMA warp follow theirs one by one.)
-    if (!bar_wait(&S.bar_done, n_win & 1u)) S.abort = 1;
-    // completions of this tile: MMA barriers 4 (columns 0,2,4,6) + 3 (1,3,5); weight barriers 4 + 3; window / done 1
-    n_mma[0] += 4u; n_mma[1] += 3u; n_w[0] += 4u; n_w[1] += 3u; n_win += 1u;
-    tc::fence_after_sync();
-    // the window and both weight buffers are free: the next tile's loads fly while the accumulators are drained
-    if (producer_warp && tile + gridDim.x < n_tiles) {
-      if (elect_one()) issue_tile_loads(tile + gridDim.x);
-      __syncwarp();
-    }
-    // ---- epilogue: warps 0-3 take output rows 0 and 2, warps 4-7 rows 1 and 3; a thread owns one pixel (= TMEM lane)
-    const uint32_t lane_base = tmem + ((uint32_t)(32 * (warp & 3)) << 16);
-    const int m = 32 * (warp & 3) + ln;
-    for (int r = warp >> 2; r < kTH; r += 2) {
-      uint32_t dreg[kC];
-      tc::tmem_ld16(lane_base + (uint32_t)(r * kC), dreg);
-      tc::tmem_ld16(lane_base + (uint32_t)(r * kC + 16), dreg + 16);
-      tc::wait_ld();
-      arm_accumulator(lane_base + (uint32_t)(r * kC), S.bias);  // folded bias: the next tile's MMAs all accumulate
-      const int y = y0 + r, x = x0 + m;
-      if (y < a.H && x < a.W) {
-        float acc[kC];
-#pragma unroll
-        for (int k = 0; k < kC; ++k) acc[k] = __uint_as_float(dreg[k]);
-        const int64_t pix = (img * a.H + y) * a.W + x;
-        conv_epilogue<EPI>(acc, a.residual, pix, a.out_act, a.out_rgb, S.out_w, S.out_b);
-      }
-    }
-    tc::wait_st();
-    tc::fence_before_sync();
-    __syncthreads();  // accumulators re-armed and drained by everyone before the next tile's MMAs
-    tc::fence_after_sync();
+    tc::reg_fence(acc, kTH * 16);
     if (S.abort) break;
+    if (tile + gridDim.x < n_tiles) load_tile_start(tile + gridDim.x);
+    // ---- epilogue from the registers: this thread's pixels x0 + 64 * wgp + 16 * wq + {g, g + 8}
+    const int xa = x0 + 64 * wgp + 16 * wq + g, xb = xa + 8;
+#pragma unroll
+    for (int r = 0; r < kTH; ++r) {
+      const int y = y0 + r;
+      const int64_t row = (img * a.H + y) * a.W;
+      const bool yok = y < a.H;
+      conv_epilogue_frag<EPI>(acc + 16 * r, a, row + xa, yok && xa < a.W, row + xb, yok && xb < a.W, t, S.out_w, S.out_b);
+    }
   }
+  if (!TMA) cp_async_wait<0>();
   if (S.abort && tid == 0 && a.status) atomicExch(a.status, 2);
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tmem, kTmemCols);
 }
+
+template <int EPI>
+__global__ void __launch_bounds__(kConvThreads, 1) dec_conv7_tma_kernel(const __grid_constant__ ConvArgsTma P) {
+  conv7_body<EPI, true>(P.a, &P.in_map);
+}
+template <int EPI>
+__global__ void __launch_bounds__(kConvThreads, 1) dec_conv7_tc_kernel(const ConvArgs a) {
+  conv7_body<EPI, false>(a, nullptr);
+}
+
 
 // ------------------------------------------------------------------ 7x7 conv on the CUDA cores (fp32 reference)
 // Same inputs, outputs and epilogues as dec_conv7_tc_kernel; one thread per output pixel, the weights of one tap row

@@ -1,91 +1,123 @@
-// tc_mlp.cuh -- tiny-MLP layers on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a only.
+// tc_mlp.cuh -- tiny-MLP layers on Hopper's warp-group tensor cores (wgmma), sm_90a.
 //
-// A tile is 128 rows (= 4 warps x 32 lanes; in the render kernel 4 rays x 32 samples).  Each row lives in one TMEM
-// lane:  activations A (fp32, read by the MMA as TF32) in columns [A_hi | A_lo], the fp32 accumulator D in another
-// column range.  Weights are the B operand, staged once per CTA in shared memory in the canonical K-major
-// no-swizzle ("interleave") UMMA layout.  fp32 accuracy is recovered with the 3xTF32 split
+// A tile is 128 rows held one per thread by a warp group.  A layer D[128 x N] = A[128 x K] * W^T: every thread writes its
+// row to the group's shared-memory stage, the group runs two m64nNk8 TF32 wgmma tiles with A fragments loaded from the
+// stage into registers and B = the weights in shared memory (canonical K-major no-swizzle layout), the accumulators go
+// back to the stage and every thread reads its own row of D.
+// fp32 accuracy is recovered with the 3xTF32 split
 //     x*w ~= x_hi*w_hi + x_lo*w_hi + x_hi*w_lo        (x_hi = x with the 13 low mantissa bits cleared)
-// i.e. three tcgen05.mma per 8-wide k-step accumulating into the same TMEM columns; the dropped x_lo*w_lo term is
-// ~2^-22 relative.  One elected thread issues the MMAs; completion is signalled with tcgen05.commit on an mbarrier.
+// i.e. three wgmma per 8-wide k-step accumulating into the same registers; the dropped x_lo*w_lo term is ~2^-22 relative.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-
-#ifndef NFF_MBAR_HINT
-#define NFF_MBAR_HINT 0  // ns; 0 = plain try_wait
-#endif
 
 namespace tc {
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers stay untouched by other instructions while a wgmma that writes them is in flight
+__device__ __forceinline__ void reg_fence(float* d, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// Bounded wait: returns false instead of hanging the GPU if the MMA never signals (a wrong descriptor must show up
-// as a failed test, not as a wedged box).
+// Bounded wait: returns false instead of hanging the GPU if a copy never completes (a wrong tensor map must show up as a
+// failed status, not as a wedged GPU).
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
   for (int it = 0; it < (1 << 20); ++it) {
     uint32_t ok;
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-#if NFF_MBAR_HINT
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"  // suspend-time hint: sleep in hardware, not in the loop
-#else
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-#endif
         "selp.b32 %0, 1, 0, p;\n\t}"
         : "=r"(ok)
-#if NFF_MBAR_HINT
-        : "r"(addr), "r"(parity), "r"((uint32_t)NFF_MBAR_HINT)
-#else
         : "r"(addr), "r"(parity)
-#endif
         : "memory");
     if (ok) return true;
   }
   return false;
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T, TF32 inputs, fp32 accumulate, M = 128
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ uint32_t elect_one() {  // one lane of the converged warp (the same one every time)
+  uint32_t pred;
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred P;\n\t"
+      "elect.sync _|P, 0xffffffff;\n\t"
+      "selp.b32 %0, 1, 0, P;\n\t}"
+      : "=r"(pred));
+  return pred;
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
+
+// wgmma with fp32 accumulators d (this thread's N/2 fragment registers of an m64 tile); scale-d = 1: D += A * B
+// (accumulators are zeroed or preset by the caller).
+// "+f" operands d[i .. i + 8)
+#define TC_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define TC_D16(i) TC_D8(i), TC_D8(i + 8)
+#define TC_D32(i) TC_D16(i), TC_D16(i + 16)
+__device__ __forceinline__ void wgmma_tf32_m64n16(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\twgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+               : TC_D8(0)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void wgmma_tf32_m64n32(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\twgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+               : TC_D16(0)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32_m64n48(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\twgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p, 1, 1;\n\t}"
+               : TC_D16(0), TC_D8(16)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32_m64n64(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+               : TC_D32(0)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_bf16_m64n32(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+               : TC_D16(0)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_bf16_m64n64(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : TC_D32(0)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_bf16_m64n96(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\twgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+               : TC_D32(0), TC_D16(32)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_bf16_m64n128(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+               : TC_D32(0), TC_D32(32)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t b_desc) {
+  static_assert(N == 16 || N == 32 || N == 48 || N == 64, "tf32 tile widths");
+  if constexpr (N == 16) wgmma_tf32_m64n16(d, a, b_desc);
+  else if constexpr (N == 32) wgmma_tf32_m64n32(d, a, b_desc);
+  else if constexpr (N == 48) wgmma_tf32_m64n48(d, a, b_desc);
+  else wgmma_tf32_m64n64(d, a, b_desc);
 }
 
 // ------------------------------------------------------------------------------------------- operand layouts
@@ -110,83 +142,102 @@ __device__ __forceinline__ void stage_b_tile(float* hi, float* lo, const float* 
     lo[off] = v - h;  // exact in fp32; the tensor core truncates it to TF32 (error ~2^-22 |v|)
   }
 }
-// 64-bit shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type=SWIZZLE_NONE(0) [61,64)
-__device__ __forceinline__ uint64_t b_desc(const float* tile, int k_pad) {
-  const uint64_t addr = (uint64_t)((smem_u32(tile) & 0x3ffffu) >> 4);
-  const uint64_t lbo = 128u >> 4;
-  const uint64_t sbo = (uint64_t)((k_pad >> 2) * 128) >> 4;
-  return addr | (lbo << 16) | (sbo << 32) | (1ull << 46);
-}
-// 32-bit instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 (1<<4), A=TF32 (2<<7), B=TF32 (2<<10), both
-// K-major, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t idesc_tf32(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// 64-bit shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// base offset 0, layout_type = no swizzle (0) [62,64)
+__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 
 // ------------------------------------------------------------------------------------------------ tile ops
-// TMEM column map of one 128-row tile (kATotal = max K over the layers)
-template <int K_MAX, int N_MAX>
-struct TileCols {
-  static constexpr int a_hi = 0, a_lo = K_MAX, d = 2 * K_MAX, total = 2 * K_MAX + N_MAX;
-};
+// Row pitch (floats) of a 128-row stage holding up to W columns.
+__host__ __device__ constexpr int stage_pitch(int w) { return (w + 7) / 8 * 8 + 4; }
 
-// Every thread writes `n` (multiple of 8) activations of ITS row into A columns [k0, k0+n).
-// lane_base = tmem base | (32*(warp%4)) << 16.
+// This thread's `n` (multiple of 4) values -> its row of the stage.  row = thread index within the warp group.
 template <int K_MAX>
-__device__ __forceinline__ void store_a(uint32_t lane_base, int k0, const float* x, int n) {
+__device__ __forceinline__ void store_row(float* stage, int pitch, const float* x, int n) {
+  float4* dst = reinterpret_cast<float4*>(stage + (threadIdx.x & 127) * pitch);
 #pragma unroll
-  for (int c = 0; c < K_MAX; c += 8) {
+  for (int c = 0; c < K_MAX; c += 4)
+    if (c < n) dst[c / 4] = make_float4(x[c], x[c + 1], x[c + 2], x[c + 3]);
+}
+template <int N_MAX>
+__device__ __forceinline__ void load_row(const float* stage, int pitch, float* y, int n) {
+  const float4* src = reinterpret_cast<const float4*>(stage + (threadIdx.x & 127) * pitch);
+#pragma unroll
+  for (int c = 0; c < N_MAX; c += 4)
     if (c < n) {
-      uint32_t h[8], l[8];
+      const float4 v = src[c / 4];
+      y[c] = v.x, y[c + 1] = v.y, y[c + 2] = v.z, y[c + 3] = v.w;
+    }
+}
+
+// acc[N] += stage[128 x k_pad] * W^T, 3xTF32, by a converged warp group once the stage is full.  acc: [half][N/2]
+// fragments (rows 64*half + 16*warp + lane/4 (+8), columns 8j + 2*(lane%4) (+1)).
+template <int N>
+__device__ __forceinline__ void tile_mma(const float* stage, int pitch, int k_pad, const float* b_hi, const float* b_lo, float* acc) {
+  const int wq = (threadIdx.x >> 5) & 3, ln = threadIdx.x & 31, g = ln >> 2, t = ln & 3;
+  const uint32_t sbo = (uint32_t)(k_pad >> 2) * 128u;
+  const uint64_t dh0 = smem_desc(smem_u32(b_hi), 128u, sbo), dl0 = smem_desc(smem_u32(b_lo), 128u, sbo);
+  for (int ks = 0; ks < k_pad / 8; ++ks) {
+    uint32_t ah[2][4], al[2][4];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float v = x[c + i];
-        float vh = tf32_hi(v);
-        h[i] = __float_as_uint(vh);
-        l[i] = __float_as_uint(v - vh);
+    for (int h = 0; h < 2; ++h) {
+      const float* r0 = stage + (64 * h + 16 * wq + g) * pitch + 8 * ks + t;
+      const float* r1 = r0 + 8 * pitch;
+      const float v[4] = {r0[0], r1[0], r0[4], r1[4]};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float vh = tf32_hi(v[i]);
+        ah[h][i] = __float_as_uint(vh);
+        al[h][i] = __float_as_uint(v[i] - vh);
       }
-      tmem_st8(lane_base + (uint32_t)(k0 + c), h);
-      tmem_st8(lane_base + (uint32_t)(K_MAX + k0 + c), l);
+    }
+    const uint64_t adv = (uint64_t)((ks * 2 * 128) >> 4);  // two 16-byte K-chunks (= 2 core matrices) per k-step
+    wg_fence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      wgmma_tf32<N>(acc + h * (N / 2), ah[h], dh0 + adv);
+      wgmma_tf32<N>(acc + h * (N / 2), al[h], dh0 + adv);
+      wgmma_tf32<N>(acc + h * (N / 2), ah[h], dl0 + adv);
+    }
+    wg_commit();
+    wg_wait<0>();  // the fragment registers of this k-step are reused by the next
+  }
+  reg_fence(acc, N);
+}
+// accumulator fragments -> stage rows (each warp writes the rows of its own fragments; __syncwarp orders them after the
+// warp's fragment reads of the same rows)
+template <int N>
+__device__ __forceinline__ void tile_store_d(float* stage, int pitch, const float* acc) {
+  const int wq = (threadIdx.x >> 5) & 3, ln = threadIdx.x & 31, g = ln >> 2, t = ln & 3;
+  __syncwarp();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* r0 = stage + (64 * h + 16 * wq + g) * pitch + 2 * t;
+    float* r1 = r0 + 8 * pitch;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const float* d = acc + h * (N / 2) + 4 * j;
+      *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[0], d[1]);
+      *reinterpret_cast<float2*>(r1 + 8 * j) = make_float2(d[2], d[3]);
     }
   }
 }
 
-__device__ __forceinline__ uint32_t elect_one() {  // one lane of the converged warp (the same one every time)
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred;
-}
-// Issue one layer: D[128 x N] = A[128 x K] * W^T with the 3xTF32 split.  Called by ONE CONVERGED WARP with
-// warp-uniform arguments: the descriptors are then warp-uniform values the compiler keeps in uniform registers (where
-// tcgen05.mma takes its operands from) and one elected lane issues.  Built inside a single-thread branch instead, every
-// MMA pays a ~10-instruction register->uniform-register broadcast loop.
-template <int K_MAX>
-__device__ __forceinline__ void issue_layer(uint32_t tmem_base, int d_col, const float* b_hi, const float* b_lo, int k_pad, int n_pad,
-                                            uint64_t* bar) {
-  const uint32_t leader = elect_one();
-  const uint32_t idesc = idesc_tf32(128, n_pad);
-  // low words: start >> 4 | LBO (128 B) >> 4 << 16; high words: SBO >> 4 | version 1
-  const uint32_t h32 = ((smem_u32(b_hi) & 0x3ffffu) >> 4) | ((128u >> 4) << 16);
-  const uint32_t l32 = ((smem_u32(b_lo) & 0x3ffffu) >> 4) | ((128u >> 4) << 16);
-  const uint32_t hi32 = (uint32_t)(((k_pad >> 2) * 128) >> 4) | (1u << 14);
-  const uint32_t d = tmem_base + (uint32_t)d_col;
-  for (int ks = 0; ks < k_pad / 8; ++ks) {
-    const uint32_t adv = (uint32_t)(ks * 2 * 128) >> 4;  // two 16-byte K-chunks (= 2 core matrices) per k-step
-    const uint32_t a_hi = tmem_base + (uint32_t)(ks * 8), a_lo = tmem_base + (uint32_t)(K_MAX + ks * 8);
-    const uint64_t dh = ((uint64_t)hi32 << 32) | (h32 + adv), dl = ((uint64_t)hi32 << 32) | (l32 + adv);
-    if (leader) {
-      mma_tf32_ts(d, a_hi, dh, idesc, ks != 0);
-      mma_tf32_ts(d, a_lo, dh, idesc, 1);
-      mma_tf32_ts(d, a_hi, dl, idesc, 1);
-    }
-  }
-  if (leader) mma_commit(bar);
-  __syncwarp();
+// One layer of the tile: x (this thread's k_pad inputs) -> out (its N outputs, no bias).  All 128 threads of the warp
+// group; `sync` is the group's barrier.
+template <int K_MAX, int N, class Sync>
+__device__ __forceinline__ void tile_layer(float* stage, int pitch, const float* x, int k_pad, const float* b_hi, const float* b_lo,
+                                           float* out, Sync&& sync) {
+  store_row<K_MAX>(stage, pitch, x, k_pad);
+  sync();  // every row is in; also: every thread has read its previous D row
+  float acc[N];
+#pragma unroll
+  for (int i = 0; i < N; ++i) acc[i] = 0.0f;
+  tile_mma<N>(stage, pitch, k_pad, b_hi, b_lo, acc);
+  tile_store_d<N>(stage, pitch, acc);
+  sync();
+  load_row<N>(stage, pitch, out, N);
 }
 
 }  // namespace tc

@@ -8,7 +8,7 @@ modules, so that the parity tests read like the reference's own tests and a refe
   cameras/rays.py:252           RayBundle                      RayBundle
   field_components/encodings.py:311  HashEncoding(implementation=) HashEncoding      (forward -> hashgrid_fwd kernel)
   field_components/encodings.py:760  SHEncoding(levels=4)      SHEncoding        (forward -> sh4_fwd kernel)
-  field_components/mlp.py:60    MLP(implementation=)           MLP               (forward -> tcgen05 mlp_fwd kernel)
+  field_components/mlp.py:60    MLP(implementation=)           MLP               (forward -> wgmma mlp_fwd kernel)
   model_components/ray_samplers.py:255  PDFSampler             PDFSampler        (-> pdf_resample kernel)
   model_components/ray_samplers.py:56,135,838  Spaced/Uniform/.../PowerSampler  same names (-> spaced_sample kernel)
   cameras/rays.py:33,127        Frustums, RaySamples           same names (get_positions / get_weights kernels)
@@ -16,7 +16,7 @@ modules, so that the parity tests read like the reference's own tests and a refe
   models/neurad.py:165          NeuRADModel.get_nff_outputs /  NeuRADModel       (-> fused nff_render_fwd kernel)
                                 get_outputs_for_camera_ray_bundle / decode_features (lidar half)
   field_components/neurad_encoding.py:85  NeuRADHashEncoding   NeuRADHashEncoding (-> neurad_encoding_fwd kernel)
-  fields/neurad_field.py:76,186  NeuRADField, NeuRADProposalField  same names (encoding + tcgen05 MLPs + head kernels)
+  fields/neurad_field.py:76,186  NeuRADField, NeuRADProposalField  same names (encoding + wgmma MLPs + head kernels)
   model_components/ray_samplers.py:569  ProposalNetworkSampler  ProposalNetworkSampler (stage kernels, density_fns)
                                 NeuRADModel.field / .proposal_fields / .sampler / .density_fns as in neurad.py:180-248;
                                 get_nff_outputs(fused=False) walks these modules like the reference does
@@ -49,7 +49,7 @@ def get_backend(device: torch.device) -> B200Backend:
     """One B200Backend (= one b200nerf_ctx) per CUDA device and process."""
     device = torch.device(device)
     if device.type != "cuda":
-        raise RuntimeError("the b200 implementation runs on CUDA (sm_100a) devices only; there is no CPU fallback")
+        raise RuntimeError("the b200 implementation runs on CUDA (sm_90a) devices only; there is no CPU fallback")
     idx = device.index if device.index is not None else torch.cuda.current_device()
     if idx not in _BACKENDS:
         _BACKENDS[idx] = B200Backend(torch.device("cuda", idx))
@@ -249,7 +249,7 @@ class MLP(nn.Module):
     def forward(self, in_tensor: Tensor) -> Tensor:
         be = get_backend(in_tensor.device)
         wb = [t for l in self.layers for t in (l.weight, l.bias)]
-        if _needs_grad(in_tensor, *wb):  # MLP backward operators (dX on tcgen05, dW / db)
+        if _needs_grad(in_tensor, *wb):  # MLP backward operators (dX on wgmma, dW / db)
             y = AG.MlpFn.apply(be, in_tensor.reshape(-1, in_tensor.shape[-1]).contiguous(), *wb).reshape(*in_tensor.shape[:-1], self.out_dim)
         else:
             with torch.no_grad():
@@ -789,7 +789,7 @@ class BasicBlock(nn.Module):
 
     def forward(self, x: Tensor) -> Tensor:
         """cnns.py:45-46.  Only reached through RGBDecoder.forward(impl="torch") (training): the inference path evaluates
-        the whole decoder with the fused tcgen05 convolutions and never calls the blocks one by one."""
+        the whole decoder with the fused wgmma convolutions and never calls the blocks one by one."""
         return self.final_activation(self.res_branch(x) + self.main_branch(x))
 
 
@@ -1142,7 +1142,7 @@ class NeuRADModel(nn.Module):
     def decode_features(self, features: Tensor, patch_size: Optional[Tuple[int, int]] = None, is_lidar: Optional[Tensor] = None,
                         intensity_for_cam: bool = False):
         """neurad.py:337-366.  With `patch_size` (the reference's signature) returns (rgb, intensity, ray_drop_logits):
-        lidar rays (`is_lidar` [N,1]) go through `lidar_decoder` (MLP 48->32->32->2 on the tcgen05 operator, intensity =
+        lidar rays (`is_lidar` [N,1]) go through `lidar_decoder` (MLP 48->32->32->2 on the wgmma operator, intensity =
         sigmoid), camera rays are reshaped to patches [B,ph,pw,C] and decoded by `rgb_decoder` to [B,3ph,3pw,3]
         (channels-last in and out: the reference's two permutes cancel).  Without `patch_size`: the lidar half only,
         (intensity, ray_drop_logits) for all rows."""
@@ -1175,7 +1175,7 @@ class NeuRADModel(nn.Module):
         rgb = None
         if cam_features.numel() > 0:
             patches = cam_features.reshape(-1, *patch_size, cam_features.shape[-1])
-            # inference: the tcgen05 decoder kernels.  Training (BatchNorm batch statistics + autograd): explicitly the torch
+            # inference: the wgmma decoder kernels.  Training (BatchNorm batch statistics + autograd): explicitly the torch
             # modules, as the reference does -- the native decoder has no backward yet (DESIGN.md section 8)
             rgb = self.rgb_decoder(patches, impl="torch" if (self.rgb_decoder.training and torch.is_grad_enabled()) else "tc")
         return rgb, intensity, ray_drop_logit

@@ -8,7 +8,7 @@ CPU it reproduces the reference bit for bit wherever the reference itself is det
 
 Who may use it: ``tests/``, ``__graft_entry__.smoke()`` and the ``cpu_baseline`` / ``--impl reference`` legs of
 ``bench.py`` -- as the checker or the timed baseline, never as the product.  Nothing under
-``neurad-studio_b200/`` imports this module; the product path is the sm_100a CUDA library and it fails loudly
+``neurad-studio_b200/`` imports this module; the product path is the sm_90a CUDA library and it fails loudly
 when that library is missing.
 
 Pinning status: the reference's own tests hold NO golden vector for this path (SURVEY.md section 8c), so the

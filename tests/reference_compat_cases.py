@@ -1,6 +1,6 @@
 """The reference's own unit tests for the modules on this path (tests/model_components/test_ray_sampler.py,
 test_renderers.py, tests/cameras/test_rays.py, tests/utils/test_math.py, tests/field_components/test_encodings.py,
-test_mlp.py), with the imports switched to the B200 mirror -- same names, same bodies, `dev` added.  SURVEY.md 8c lists
+test_mlp.py), with the imports switched to the library's mirror -- same names, same bodies, `dev` added.  SURVEY.md 8c lists
 them as the closest thing to fixtures the reference has ("API smoke"); the value checks live in the parity suites."""
 import pytest
 import torch

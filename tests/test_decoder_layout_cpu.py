@@ -1,5 +1,5 @@
-"""CPU: numpy model of the shared-memory layouts and UMMA descriptor arithmetic of dec_conv7_tc_kernel
-(neurad-studio_b200/csrc/rgb_decoder.cuh).  tcgen05 cannot run here, but the address arithmetic can: the model reads
+"""CPU: numpy model of the shared-memory layouts and GMMA descriptor arithmetic of dec_conv7_tc_kernel
+(neurad-studio_b200/csrc/rgb_decoder.cuh).  wgmma cannot run here, but the address arithmetic can: the model reads
 the A / B operands through the canonical K-major no-swizzle descriptor rule
     element (row, k) of a bf16 operand = start + (row/8)*SBO + (k/8)*LBO + (row%8)*16 + (k%8)*2   [bytes]
 exactly as the kernel programs them (plane-shifted activation windows, tap-column weight images with the tiles of one

@@ -67,7 +67,7 @@ def _check_against(out, ref, beta):
 @pytest.mark.parametrize("mode", ["lane", "split", "tc", "ffma"])
 @pytest.mark.parametrize("name", ["nff_static.npz", "nff_actors.npz", "nff_sharp.npz"])
 def test_fused_render_matches_reference_golden(backend, name, mode):
-    """All kernel variants: ray-per-lane + tcgen05 (default), warp-per-ray + tcgen05, warp-per-ray + CUDA-core fp32."""
+    """All kernel variants: ray-per-lane + wgmma (default), warp-per-ray + wgmma, warp-per-ray + CUDA-core fp32."""
     meta, g = load_golden(name)
     cfg = cfg_from_meta(meta)
     p, r, ref = g["param"], g["ray"], g["ref"]
@@ -354,11 +354,11 @@ def test_errors_are_loud(backend):
     assert fresh.render(empty)["features"].shape[0] == 0
 
 
-# ---------------------------------------------------------------------------------------- tensor-core MLP (tcgen05)
+# ---------------------------------------------------------------------------------------- tensor-core MLP (wgmma)
 @pytest.mark.parametrize("dims", [(32, 32, 33), (48, 32, 32, 32), (48, 32, 32, 2), (32, 32), (40, 24, 17), (32, 64, 4), (64, 64, 64, 64), (50, 57, 3)])
 @pytest.mark.parametrize("n_rows", [1000, 128 * 300 + 5])
 def test_mlp_fwd_tensor_core_vs_fp32(backend, dims, n_rows):
-    """MLP.forward on tcgen05 with the 3xTF32 split vs a plain fp32 (float64-accumulated) reference of the same op:
+    """MLP.forward on wgmma with the 3xTF32 split vs a plain fp32 (float64-accumulated) reference of the same op:
     NeuRAD's three MLP shapes (mlp_geo 32-32-33, mlp_feature 48-32-32-32, lidar_decoder 48-32-32-2) on the 48-column
     tile; BASELINE config 1's 32-64-4 and other <= 64-wide shapes on the 64-column tile."""
     gen = torch.Generator().manual_seed(sum(dims) + n_rows)
@@ -626,7 +626,7 @@ def _decoder_golden():
 @pytest.mark.parametrize("impl", ["ref", "tc", "tc_ldgsts"])
 def test_rgb_decoder_matches_reference_golden(backend, impl):
     """NeuRADModel.rgb_decoder (1x1 conv, 4 BasicBlocks with BatchNorm, 3x transposed conv, 1x1 conv + sigmoid) on the
-    reference's own output for a 2 x 19 x 45 feature image: CUDA-core fp32 pipeline and tcgen05 (bf16 hi/lo split)
+    reference's own output for a 2 x 19 x 45 feature image: CUDA-core fp32 pipeline and wgmma (bf16 hi/lo split)
     pipeline, both within the 1e-4 parity bar."""
     p, feats, ref = _decoder_golden()
     backend.set_rgb_decoder(p)
@@ -640,7 +640,7 @@ def test_rgb_decoder_matches_reference_golden(backend, impl):
 
 def test_rgb_decoder_tensor_core_multi_tile(backend):
     """Several strips / row tiles / images, ragged edges (width 300 -> 900 = 7 x 128 + 4, heights not multiples of 3):
-    tcgen05 path vs the CPU oracle and vs the in-library CUDA-core path."""
+    wgmma path vs the CPU oracle and vs the in-library CUDA-core path."""
     from oracle import decoder_oracle as D
 
     p = D.random_decoder_params(seed=21)

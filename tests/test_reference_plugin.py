@@ -92,7 +92,7 @@ def test_registry_discovers_the_method(plugin):
     from nerfstudio.engine.trainer import TrainerConfig
     from nerfstudio.models.neurad import NeuRADModelConfig
 
-    assert "neurad-b200" in methods and "B200" in descriptions["neurad-b200"]
+    assert "neurad-b200" in methods and "H100" in descriptions["neurad-b200"]
     cfg = methods["neurad-b200"]
     assert isinstance(cfg, TrainerConfig) and cfg.method_name == "neurad-b200"
     mc = cfg.pipeline.model

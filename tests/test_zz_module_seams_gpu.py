@@ -2,8 +2,7 @@
 through the C ABI) and of the backward operators / training-mode semantics (SURVEY 8f row f2), against the reference's
 own per-stage goldens, gradient goldens (its autograd) and stratified-sampling goldens, and against the fused renderer.
 
-Every test here has run green on a B200 (round-1 driver run, round-2 sessions); the same bodies run in the CPU container
-over tests/fake_backend.py (tests/test_module_glue_cpu.py)."""
+The same bodies run in the CPU container over tests/fake_backend.py (tests/test_module_glue_cpu.py)."""
 import pytest
 
 from tests import module_seam_cases as C

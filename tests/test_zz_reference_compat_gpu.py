@@ -1,6 +1,5 @@
-"""GPU: the reference's own unit tests for the modules on this path, run against the B200 mirror (bodies in
-tests/reference_compat_cases.py; CPU twins over the fake backend in tests/test_reference_compat_cpu.py).  Green on a B200
-since the round-1 driver run."""
+"""GPU: the reference's own unit tests for the modules on this path, run against the library's mirror (bodies in
+tests/reference_compat_cases.py; CPU twins over the fake backend in tests/test_reference_compat_cpu.py)."""
 import pytest
 
 from tests import reference_compat_cases as R

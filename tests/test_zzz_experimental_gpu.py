@@ -1,6 +1,5 @@
-"""GPU: the tcgen05 split-K weight-gradient operator (`b200nerf_linear_wgrad_tc`).  Written at the end of round 1 and marked
-xfail until it had run on a B200; all 18 cases passed there (round-1 driver run and round 2's sessions), so these are
-ordinary tests now.  The file still sorts last (a faulting kernel here cannot disturb the suites before it)."""
+"""GPU: the wgmma split-K weight-gradient operator (`b200nerf_linear_wgrad_tc`), checked like any other
+operator although the CUDA-core twin stays the default.  The file still sorts last (a faulting kernel here cannot disturb the suites before it)."""
 import pytest
 import torch
 
@@ -15,7 +14,7 @@ def rel_to_max(a, b):
 @pytest.mark.parametrize("k,n,relu", [(32, 33, False), (32, 32, True), (48, 32, False), (64, 64, True), (6, 1, False), (50, 57, True)])
 @pytest.mark.parametrize("rows", [48 * 5, 48 * 300 + 17, 5])
 def test_linear_wgrad_tensor_core_twin(k, n, relu, rows):
-    """b200nerf_linear_wgrad_tc (tcgen05 split-K, 3xTF32) against fp64 torch and against the CUDA-core operator."""
+    """b200nerf_linear_wgrad_tc (wgmma split-K, 3xTF32) against fp64 torch and against the CUDA-core operator."""
     from neurad_studio_b200.backend import B200Backend
 
     be = B200Backend(torch.device("cuda", 0))
