@@ -521,13 +521,18 @@ class B200Backend:
                             ddensity: Optional[torch.Tensor] = None, flip: Optional[torch.Tensor] = None) -> None:
         """Backward of neurad_encoding: scatter-adds into grads["static"] [L*T,F], grads["actors"] (list of per-actor
         [La*Ta,F] tensors or None) and, in density mode (density + ddensity given), grads["decoder"] [L*F]."""
+        # the mode is decided from the arguments here: an empty batch's tensors reach the library as NULL pointers
+        if (dfeatures is None) == (ddensity is None) or (ddensity is not None and density is None):
+            raise ValueError("pass either dfeatures or (density, ddensity)")
+        if grads.get("decoder") is not None and ddensity is None:
+            raise ValueError('grads["decoder"] belongs to the density mode')
         m = self._dev(mean)
         n, s = m.shape[0], m.shape[1]
         m = m.reshape(n, s, 3)
         sd = self._dev(std).reshape(n, s)
         t = self._ray_times(times, n)
         fl = None if flip is None else self._dev(flip).reshape(n)
-        df = None if dfeatures is None else self._dev(dfeatures).reshape(n * s, -1)
+        df = None if dfeatures is None else self._dev(dfeatures).reshape(n * s, dfeatures.shape[-1])  # (n * s may be 0)
         de = None if density is None else self._dev(density).reshape(n, s)
         dd = None if ddensity is None else self._dev(ddensity).reshape(n, s)
         for g in [grads.get("static"), grads.get("decoder")] + list(grads.get("actors") or []):
@@ -550,7 +555,7 @@ class B200Backend:
         sd = self._dev(std).reshape(n, s)
         t = self._ray_times(times, n)
         fl = None if flip is None else self._dev(flip).reshape(n)
-        df = self._dev(dfeatures).reshape(n * s, -1)
+        df = self._dev(dfeatures).reshape(n * s, dfeatures.shape[-1])
         r6, ps = self._dev(rotations_6d), self._dev(positions)
         for g_ in (grad_rotations_6d, grad_positions):
             assert g_.is_contiguous() and g_.dtype == torch.float32 and g_.device == self.device

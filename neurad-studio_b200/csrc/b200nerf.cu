@@ -1578,8 +1578,10 @@ int b200nerf_neurad_encoding_fwd(b200nerf_ctx* c, int field, const float* mean, 
   DeviceGuard g(c->device);
   EncodingArgs a{mean, std, times, directions, flip, features, density, directions_out, actor_id, n_rays, n_samples,
                  directions_per_ray ? 1 : 0};
-  if (!launch_neurad_encoding_fwd(fg, c->actors, a, (cudaStream_t)stream))
+  cudaError_t opt_in = cudaSuccess;
+  if (!launch_neurad_encoding_fwd(fg, c->actors, a, (cudaStream_t)stream, opt_in))
     return fail(B200NERF_ERR_UNSUPPORTED, "encoding forward: 4 or 1 features per level, at most 8 levels");
+  CUDA_TRY(opt_in);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -1653,13 +1655,18 @@ int b200nerf_neurad_encoding_bwd(b200nerf_ctx* c, int field, const float* mean, 
   REQUIRE(field >= 0 && field < 3, "field must be B200NERF_FIELD_MAIN / PROP0 / PROP1");
   if (!c->have_field[field]) return fail(B200NERF_ERR_STATE, "b200nerf_set_field_grids was not called for this field");
   REQUIRE(n_rays >= 0 && n_samples >= 1, "bad sample grid");
-  REQUIRE((dfeatures != nullptr) != (ddensity != nullptr), "pass either dfeatures or (density, ddensity)");
-  REQUIRE(!ddensity || density, "density mode needs the forward density");
+  // An empty batch's input tensors may have NULL data pointers, so a missing pointer only counts when there are rays;
+  // every other check holds for empty batches too.
+  const bool empty = n_rays == 0;
+  REQUIRE(!(dfeatures && ddensity), "pass either dfeatures or (density, ddensity)");
+  REQUIRE(empty || dfeatures || ddensity, "pass either dfeatures or (density, ddensity)");
+  REQUIRE(empty || !ddensity || density, "density mode needs the forward density");
   const FieldGrids& fg = c->fields[field];
   if (ddensity && !fg.decoder) return fail(B200NERF_ERR_STATE, "b200nerf_set_proposal_decoder was not called for this field");
-  REQUIRE(!grad_decoder || ddensity, "grad_decoder belongs to the density mode");
+  REQUIRE(!grad_decoder || ddensity || empty, "grad_decoder belongs to the density mode");
+  REQUIRE(!grad_decoder || !dfeatures, "grad_decoder belongs to the density mode");
   if (c->actors.n_actors > kModMaxActors) return fail(B200NERF_ERR_UNSUPPORTED, "more than 64 actors");
-  if (n_rays == 0) return 0;
+  if (empty) return 0;
   REQUIRE(mean && std, "NULL argument");
   REQUIRE(c->actors.n_actors == 0 || times, "times are required when the scene has actors");
   DeviceGuard g(c->device);
@@ -1671,8 +1678,10 @@ int b200nerf_neurad_encoding_bwd(b200nerf_ctx* c, int field, const float* mean, 
   }
   EncodingBwdArgs a{mean, std, times, flip, dfeatures, density, ddensity, grad_static_table, d_ptrs, grad_decoder, n_rays,
                     n_samples};
-  if (!launch_neurad_encoding_bwd(fg, c->actors, a, (cudaStream_t)stream))
+  cudaError_t opt_in = cudaSuccess;
+  if (!launch_neurad_encoding_bwd(fg, c->actors, a, (cudaStream_t)stream, opt_in))
     return fail(B200NERF_ERR_UNSUPPORTED, "encoding backward: features mode needs 4 features / level, density mode 1 (<= 8 levels)");
+  CUDA_TRY(opt_in);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

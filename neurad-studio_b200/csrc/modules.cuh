@@ -114,14 +114,16 @@ __global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_fwd_kernel(con
     }
   }
 }
-// Host dispatch (false: grid shapes b200nerf_set_field_grids does not admit).
-inline bool launch_neurad_encoding_fwd(const FieldGrids& fg, const Actors& A, const EncodingArgs& a, cudaStream_t stream) {
+// Host dispatch (false: grid shapes b200nerf_set_field_grids does not admit).  `err`: the shared-memory opt-in's error,
+// if it failed (the launch is then skipped).
+inline bool launch_neurad_encoding_fwd(const FieldGrids& fg, const Actors& A, const EncodingArgs& a, cudaStream_t stream, cudaError_t& err) {
+  err = cudaSuccess;
   const unsigned grid = (unsigned)((a.n_rays + kModWarps - 1) / kModWarps);
   if (grid == 0) return true;
   auto launch = [&](auto kernel, int F) {
     const size_t smem = sizeof(float) * kModWarps * 32 * (8 * F + 1) + sizeof(ActorFrame) * kModWarps * (size_t)A.n_actors;
-    if (smem > kSmemOptIn) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kernel<<<grid, kModWarps * 32, smem, stream>>>(fg, A, a);
+    if (smem > kSmemOptIn) err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) kernel<<<grid, kModWarps * 32, smem, stream>>>(fg, A, a);
   };
   if (encode_bwd_fast_ok(fg, A.n_actors, 4))
     launch(neurad_encoding_fwd_kernel<4>, 4);
@@ -311,19 +313,24 @@ __global__ void __launch_bounds__(kBwdThreads, MODE == 1 ? NFF_BWD_MINB_F4 : 4) 
 }
 // Host dispatch; false when the bound grids do not have the shapes the variants are written for (cannot happen behind
 // b200nerf_set_field_grids, which admits NeuRAD's shapes only -- the caller turns it into an error instead of guessing).
-inline bool launch_neurad_encoding_bwd(const FieldGrids& fg, const Actors& A, const EncodingBwdArgs& a, cudaStream_t stream) {
+// `err`: the shared-memory opt-in's error, if it failed (the launch is then skipped).
+inline bool launch_neurad_encoding_bwd(const FieldGrids& fg, const Actors& A, const EncodingBwdArgs& a, cudaStream_t stream,
+                                       cudaError_t& err) {
+  err = cudaSuccess;
   const unsigned grid = (unsigned)((a.n_rays + kBwdRays - 1) / kBwdRays);
-  const size_t smem = sizeof(ActorFrame) * kBwdRays * (size_t)A.n_actors;  // <= 64 KB at kModMaxActors
+  // 64 B per ray and actor: 2 KB per actor, above the 48 KB default from 24 actors on, 128 KB at kModMaxActors
+  const size_t smem = sizeof(ActorFrame) * kBwdRays * (size_t)A.n_actors;
   if (grid == 0) return true;
-  if (!a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 4)) {
-    if (smem > kSmemOptIn) cudaFuncSetAttribute(neurad_encoding_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    neurad_encoding_bwd_kernel<1><<<grid, kBwdThreads, smem, stream>>>(fg, A, a);
-  } else if (a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 1)) {
-    if (smem > kSmemOptIn) cudaFuncSetAttribute(neurad_encoding_bwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    neurad_encoding_bwd_kernel<2><<<grid, kBwdThreads, smem, stream>>>(fg, A, a);
-  } else {
+  auto launch = [&](auto kernel) {
+    if (smem > kSmemOptIn) err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) kernel<<<grid, kBwdThreads, smem, stream>>>(fg, A, a);
+  };
+  if (!a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 4))
+    launch(neurad_encoding_bwd_kernel<1>);
+  else if (a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 1))
+    launch(neurad_encoding_bwd_kernel<2>);
+  else
     return false;
-  }
   return true;
 }
 

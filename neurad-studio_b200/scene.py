@@ -34,10 +34,12 @@ def _table(gen: torch.Generator, g: HashGridSettings, scale: float, device="cpu"
     return t * scale
 
 
-def make_trajectories(n_actors: int, duration: float = 8.0, hz: float = 10.0, seed: int = 0) -> List[dict]:
+def make_trajectories(n_actors: int, duration: float = 8.0, hz: float = 10.0, seed: int = 0, axis_aligned: bool = False) -> List[dict]:
     """Straight-line rigid actors on four lanes ahead of the ego; padded boxes never overlap (the reference's
     duplicate-hit winner is unspecified, neurad_encoding.py:256-263).  Same dict layout as the dataparsers'
-    ``metadata["trajectories"]`` (dynamic_actors.py:109-170): timestamps [T], poses [T,4,4], dims (w,l,h)."""
+    ``metadata["trajectories"]`` (dynamic_actors.py:109-170): timestamps [T], poses [T,4,4], dims (w,l,h).
+    `axis_aligned`: yaw exactly -90 degrees (rotation entries 0 / +-1), so that the world -> box transform is exact in
+    fp32 whatever the order of its operations."""
     gen = torch.Generator().manual_seed(seed + 12345)
     n_t = int(round(duration * hz)) + 1
     ts = torch.arange(n_t, dtype=torch.float64) / hz
@@ -48,7 +50,7 @@ def make_trajectories(n_actors: int, duration: float = 8.0, hz: float = 10.0, se
         x0 = 12.0 + 14.0 * slot + 3.0 * lane
         speed = (8.0, 10.0, 11.0, 9.0)[lane]
         yaw = -math.pi / 2 + 0.05 * (float(torch.rand((), generator=gen)) - 0.5)  # box y-axis (length) along +x
-        c, s = math.cos(yaw), math.sin(yaw)
+        c, s = (0.0, -1.0) if axis_aligned else (math.cos(yaw), math.sin(yaw))
         poses = torch.eye(4, dtype=torch.float32).repeat(n_t, 1, 1)
         poses[:, 0, 0], poses[:, 0, 1], poses[:, 1, 0], poses[:, 1, 1] = c, -s, s, c
         poses[:, 0, 3] = (x0 + speed * ts).float()

@@ -264,9 +264,9 @@ def encoding_bwd(cfg, params, pdf_u, field, mean, std, times, grads, dfeatures=N
     ex = _Pack()
     ex.P(mean.float().reshape(n, s, 3))
     ex.P(std.float().reshape(n, s))
-    ex.P(None if times is None else times.float().reshape(n, -1)[:, 0])
+    ex.P(None if times is None else times.float().reshape(n) if times.numel() == n else times.float().reshape(n, -1)[:, 0])
     ex.P(None if flip is None else flip.float().reshape(n))
-    ex.P(None if dfeatures is None else dfeatures.float().reshape(n * s, -1))
+    ex.P(None if dfeatures is None else dfeatures.float().reshape(n * s, dfeatures.shape[-1]))
     ex.P(None if density is None else density.float().reshape(n, s))
     ex.P(None if ddensity is None else ddensity.float().reshape(n, s))
     for t in (grads.get("static"),):
