@@ -244,17 +244,15 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
                                                                                       const float* __restrict__ handoff) {
   extern __shared__ __align__(128) unsigned char smem_shade[];
   TcShared* tcs = reinterpret_cast<TcShared*>(smem_shade);
-  float* geo_park = reinterpret_cast<float*>(smem_shade + tc_smem_bytes(kLaneThreads));
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
-  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
+  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads, true);
   tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
   MlpLaneTc mlp;
-  mlp.core.t = tcs;
-  mlp.core.stage = reinterpret_cast<float*>(smem_shade + kTcBytes) + group * kTcStageFloats;
-  mlp.core.bar_id = 1 + group;
+  mlp.t = tcs;
+  mlp.panel_ = reinterpret_cast<float*>(smem_shade + kTcBytes);
+  mlp.bar_id = 1 + group;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
-  mlp.geo_park = NFF_PANEL_GLOBAL ? sc.panel : geo_park;
   mlp.sh_tcnn = LAYOUT;
   // a warp group (one 128-row tensor-core tile) renders 4 consecutive patches; the groups of a CTA only meet at the two
   // block barrier before the loop, inside it they synchronise among their own 4 warps (named barriers).
@@ -286,17 +284,15 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_
                                                                           float* __restrict__ scratch) {
   extern __shared__ __align__(128) unsigned char smem_lane[];
   TcShared* tcs = reinterpret_cast<TcShared*>(smem_lane);
-  float* geo_park = reinterpret_cast<float*>(smem_lane + tc_smem_bytes(kLaneThreads));
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
-  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
+  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads, true);
   tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
   MlpLaneTc mlp;
-  mlp.core.t = tcs;
-  mlp.core.stage = reinterpret_cast<float*>(smem_lane + kTcBytes) + group * kTcStageFloats;
-  mlp.core.bar_id = 1 + group;
+  mlp.t = tcs;
+  mlp.panel_ = reinterpret_cast<float*>(smem_lane + kTcBytes);
+  mlp.bar_id = 1 + group;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
-  mlp.geo_park = NFF_PANEL_GLOBAL ? sc.panel : geo_park;
   for (int64_t unit = blockIdx.x; unit < lane_units(P); unit += gridDim.x) {
     int64_t ray;
     const bool active = lane_unit_ray(P, unit, tid, &ray);
@@ -1028,13 +1024,13 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
   CUDA_TRY(cudaMalloc((void**)&c->d_status, sizeof(int)));
   CUDA_TRY(cudaMemset(c->d_status, 0, sizeof(int)));
   CUDA_TRY(cudaFuncSetAttribute(nff_render_lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)lane_tc_smem_bytes()));
   c->lane_ctas = c->sm_count * (kLaneCtasPerSm > NFF_SAMPLE_CTAS ? kLaneCtasPerSm : NFF_SAMPLE_CTAS);
   CUDA_TRY(cudaMalloc((void**)&c->d_lane_scratch, sizeof(float) * lane_scratch_floats_per_cta() * c->lane_ctas));
   CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)lane_tc_smem_bytes()));
   CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)(tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads))));
+                                (int)lane_tc_smem_bytes()));
   CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<0>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));  // all L1
   CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
   CUDA_TRY(cudaMalloc((void**)&c->d_minmax, 2 * sizeof(unsigned)));
@@ -1379,7 +1375,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
   if (c->mlp_mode == 3) {
     // sampling kernel -> [33][rays] spacing edges -> shading kernel; bundles larger than the hand-over buffer are
     // rendered in slices (whole 16-row tile bands when an image_width hint is given)
-    const size_t smem = tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
+    const size_t smem = lane_tc_smem_bytes();
     int64_t slice = c->handoff_rays;
     if (rays->image_width > 0) {
       const int64_t band = (int64_t)rays->image_width * (kLaneThreads / 32);
@@ -1411,7 +1407,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       }
     }
   } else if (c->mlp_mode == 2) {
-    const size_t smem = tc_smem_bytes(kLaneThreads) + (NFF_PANEL_GLOBAL ? 0 : sizeof(float) * kNff * kLaneThreads);
+    const size_t smem = lane_tc_smem_bytes();
     int64_t need = (n_rays + kLaneThreads - 1) / kLaneThreads;
     if (rays->image_width > 0) {
       const int64_t W = rays->image_width, H = (n_rays + W - 1) / W;

@@ -25,9 +25,6 @@ namespace nff {
 #ifndef NFF_F4_WEIGHTS
 #define NFF_F4_WEIGHTS 0  // main-grid interpolation as a weighted sum over the 8 corners (weights shared by the 4 features)
 #endif
-#ifndef NFF_PANEL_GLOBAL
-#define NFF_PANEL_GLOBAL 0  // 1: feature panel / geo park in the global scratch slab instead of shared memory
-#endif
 constexpr int kLaneThreads = NFF_LANE_THREADS;  // threads (= rays in flight) per CTA (256: 2 CTAs/SM, 512: 1 CTA/SM)
 constexpr int kLaneCtasPerSm = 512 / kLaneThreads;
 constexpr int kCandFloats = 16;    // per candidate: 12 (world->box 3x4) + 3 (bounds) + 1 (actor id bits)
@@ -39,10 +36,9 @@ struct LaneScratch {
   float* bins1;  // [kS1 + 1]   spacing edges after round 0
   float* bins2;  // [kS2 + 1]   spacing edges after round 1
   float* cand;   // [kLaneMaxCand * kCandFloats]
-  float* panel;  // [kNff]      grid-feature panel / parked geo_embedding (when not kept in shared memory)
 };
 NFF_HD size_t lane_scratch_floats_per_cta() {
-  return (size_t)kLaneThreads * (kS0 + (kS1 + 1) + (kS2 + 1) + kLaneMaxCand * kCandFloats + kNff);
+  return (size_t)kLaneThreads * (kS0 + (kS1 + 1) + (kS2 + 1) + kLaneMaxCand * kCandFloats);
 }
 NFF_D LaneScratch lane_scratch_of(float* base, int cta) {
   float* p = base + (size_t)cta * lane_scratch_floats_per_cta();
@@ -51,7 +47,6 @@ NFF_D LaneScratch lane_scratch_of(float* base, int cta) {
   s.bins1 = s.w + (size_t)kS0 * kLaneThreads;
   s.bins2 = s.bins1 + (size_t)(kS1 + 1) * kLaneThreads;
   s.cand = s.bins2 + (size_t)(kS2 + 1) * kLaneThreads;
-  s.panel = s.cand + (size_t)kLaneMaxCand * kCandFloats * kLaneThreads;
   return s;
 }
 
@@ -167,8 +162,8 @@ NFF_D float lane_proposal_density(const FieldGrids& fg, const LaneScratch& sc, i
   return expf(acc);
 }
 
-// F = 4 grid into the CTA's shared panel column [4l+f][tid] (rolled level loop: small code)
-NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L, Gauss g, float* x /* = panel + tid */) {
+// F = 4 grid into the CTA's shared panel column [4l+f][tid] (rolled level loop: small code); `pitch` = panel row pitch
+NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L, Gauss g, float* x /* = panel + tid */, int pitch) {
   const uint32_t maskb = gr.mask << 4;
 #pragma unroll 2
   for (int l = 0; l < L; ++l) {
@@ -197,24 +192,24 @@ NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L,
       a2 = fmaf(wk[k], v[k].z, a2);
       a3 = fmaf(wk[k], v[k].w, a3);
     }
-    x[(4 * l + 0) * kLaneThreads] = a0;
-    x[(4 * l + 1) * kLaneThreads] = a1;
-    x[(4 * l + 2) * kLaneThreads] = a2;
-    x[(4 * l + 3) * kLaneThreads] = a3;
+    x[(4 * l + 0) * pitch] = a0;
+    x[(4 * l + 1) * pitch] = a1;
+    x[(4 * l + 2) * pitch] = a2;
+    x[(4 * l + 3) * pitch] = a3;
 #else
     float f[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) f[k] = v[k].x;
-    x[(4 * l + 0) * kLaneThreads] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
+    x[(4 * l + 0) * pitch] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
 #pragma unroll
     for (int k = 0; k < 8; ++k) f[k] = v[k].y;
-    x[(4 * l + 1) * kLaneThreads] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
+    x[(4 * l + 1) * pitch] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
 #pragma unroll
     for (int k = 0; k < 8; ++k) f[k] = v[k].z;
-    x[(4 * l + 2) * kLaneThreads] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
+    x[(4 * l + 2) * pitch] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
 #pragma unroll
     for (int k = 0; k < 8; ++k) f[k] = v[k].w;
-    x[(4 * l + 3) * kLaneThreads] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
+    x[(4 * l + 3) * pitch] = fmul(trilerp_b<4>(f, c, ix, iy, iz), w);
 #endif
   }
 }
@@ -310,6 +305,7 @@ NFF_D float lane_proposal_round(const RenderParams& P, const FieldGrids& fg, con
 // ------------------------------------------------------------------------------------------- MLP policies, per lane
 // Input: the 32 grid features of this lane's sample in registers.  CUDA-core version (host emulation / fp32 mode):
 struct MlpLaneFfma {
+  static constexpr int kPitch = kLaneThreads;  // panel row pitch (floats)
   const float* w;  // packed transposed weights (nff_params.h)
   float* panel_;   // [kNff][kLaneThreads]
   int sh_tcnn = 0;  // 1: tiny-cuda-nn's SphericalHarmonics convention (nff_device.h: sh4_tcnn)
@@ -331,35 +327,175 @@ struct MlpLaneFfma {
 };
 
 #if defined(__CUDACC__)
-// Tensor-core version: tile = 128 rays x this sample index; geo_embedding is parked in shared memory for the residual.
+// Tensor-core version: the tile is the 128 rays of a warp group at this sample index, run as two independent m64 halves
+// (tile rows 64h..64h+63) that each go through all five layers with every activation in wgmma fragment registers:
+//   * layer 0 loads its A fragments straight from the grid-feature panel (rows 0..31; a row pitch of 8 mod 32 banks keeps
+//     those loads free of bank conflicts).  Layer 2's K columns 32..47, the SH encoding of the direction, come from panel
+//     rows 32..47, which the row owner writes next to its features before the group barrier;
+//   * layers 1-4 take the previous layer's accumulator registers as their A operand: their B tiles have the K rows
+//     permuted to match (tc::chained_k), so ReLU and the 3xTF32 hi/lo split work on the same registers;
+//   * accumulators start at the bias, layer 4's at bias + geo_embedding (the residual).  geo_embedding waits in the panel
+//     at the thread's own fragment positions (rows 0..31, consumed by layer 0) while layers 2-3 run;
+//   * the sdf neuron is a dot product of layer 0's fragments: 8 terms per thread, then a reduction over the quad;
+//   * one commit and one wait per layer and half, except that layer 2 issues its SH k-steps as a second group after the
+//     geo_embedding ones: as one group its 48 hi/lo operand registers next to the accumulators push the sample loop's
+//     compositing state out to local memory (ptxas: 240 B of spills, against none in the loop this way).  12 waits per
+//     sample.
+// The outputs (feature c of tile row R at panel[c][R], sdf at panel[48][R]) reach the row owner behind the second and
+// last group barrier of the sample.  Panel positions of a tile row are only ever read and written as fragments by the
+// warp whose fragments hold that row, and by the row owner on the far side of a barrier.
+constexpr int kLanePanelPitch = kLaneThreads + 8;
+constexpr int kLanePanelRows = kGeoIn + kSh + 1;  // grid features | SH | sdf
+constexpr size_t lane_tc_smem_bytes() { return (size_t)kTcBytes + sizeof(float) * kLanePanelRows * kLanePanelPitch; }
 struct MlpLaneTc {
-  MlpTc core;
-  float* geo_park;  // [kNff][kLaneThreads] shared memory: grid-feature panel first, then the parked geo_embedding
-  int sh_tcnn = 0;  // 1: tiny-cuda-nn's SphericalHarmonics convention
-  NFF_D float* panel() const { return geo_park; }
-  NFF_D void run(const float* x, const float dir[3], float& sdf, float* feat, int tid) {
-    float h[kHidden], in2[kNff + kSh];
-    core.layer<32>(0, x, h);
-    float s = core.t->b_sdf;
+  static constexpr int kPitch = kLanePanelPitch;
+  const TcShared* t;  // B tiles staged by tc_stage_weights(..., chained = true)
+  float* panel_;      // [kLanePanelRows][kPitch] shared memory
+  int bar_id;         // this warp group's named barrier
+  int sh_tcnn = 0;    // 1: tiny-cuda-nn's SphericalHarmonics convention
+  NFF_D float* panel() const { return panel_; }
+  NFF_D void group_sync() const { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); }
+
+  // acc (this thread's 16 fragment registers of one m64n32 half, preset by the caller) += A * W^T over KS k-steps of a
+  // layer with K inputs, 3xTF32; a = the A fragments, 4 per k-step; b_hi = the layer's hi B tile (lo follows it) from
+  // its first k-step on (tc::b_elem_offset: one k-step is 64 floats).
+  template <int KS, int K>
+  NFF_D static void half_mma(float* acc, const float* a, const float* b_hi) {
+    uint32_t ah[4 * KS], al[4 * KS];
 #pragma unroll
-    for (int i = 0; i < kHidden; ++i) {
-      h[i] = fmaxf(h[i], 0.0f);
-      s = fmaf(h[i], core.t->w_sdf[i], s);
+    for (int i = 0; i < 4 * KS; ++i) {
+      const float h = tc::tf32_hi(a[i]);
+      ah[i] = __float_as_uint(h);
+      al[i] = __float_as_uint(a[i] - h);
     }
-    sdf = s;
-    core.layer<32>(1, h, in2);
+    const uint32_t sbo = (uint32_t)(K / 4) * 128u;  // (K / 4) core matrices of 128 B per 8-row n block
+    const uint64_t dh = tc::smem_desc(tc::smem_u32(b_hi), 128u, sbo), dl = tc::smem_desc(tc::smem_u32(b_hi + 32 * K), 128u, sbo);
+    tc::wg_fence();
 #pragma unroll
-    for (int i = 0; i < kNff; ++i) geo_park[i * kLaneThreads + tid] = in2[i];
-    if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], in2 + kNff); else sh4(dir[0], dir[1], dir[2], in2 + kNff);
-    core.layer<48>(2, in2, h);
+    for (int ks = 0; ks < KS; ++ks) {
+      const uint64_t adv = (uint64_t)((ks * 2 * 128) >> 4);  // two 16-byte K-chunks per k-step
+      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dh + adv);
+      tc::wgmma_tf32<32>(acc, al + 4 * ks, dh + adv);
+      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dl + adv);
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    // the accumulators are read, and the operand registers may be reused, only after the wait
+    tc::reg_fence(acc, 16);
 #pragma unroll
-    for (int i = 0; i < kHidden; ++i) h[i] = fmaxf(h[i], 0.0f);
-    core.layer<32>(3, h, in2);
+    for (int i = 0; i < 4 * KS; ++i) asm volatile("" : "+r"(ah[i]), "+r"(al[i])::"memory");
+  }
+  // A fragments of k-steps [0, 4) from the accumulator fragments of the previous layer (K rows of B permuted)
+  NFF_D static void chain(float* a, const float* acc) {
 #pragma unroll
-    for (int i = 0; i < kHidden; ++i) in2[i] = fmaxf(in2[i], 0.0f);
-    core.layer<32>(4, in2, h);
+    for (int j = 0; j < 4; ++j) {
+      a[4 * j + 0] = acc[4 * j + 0];
+      a[4 * j + 1] = acc[4 * j + 2];
+      a[4 * j + 2] = acc[4 * j + 1];
+      a[4 * j + 3] = acc[4 * j + 3];
+    }
+  }
+  // A fragments of k-steps [ks0, ks0 + n) from panel rows 8 ks0 .. (p = the panel at this thread's fragment row g)
+  NFF_D static void load_a(float* a, const float* p, int q, int ks0, int n) {
 #pragma unroll
-    for (int i = 0; i < kNff; ++i) feat[i] = geo_park[i * kLaneThreads + tid] + h[i];
+    for (int i = 0; i < n; ++i) {
+      const float* r = p + (8 * (ks0 + i) + q) * kPitch;
+      a[4 * i + 0] = r[0];
+      a[4 * i + 1] = r[8];
+      a[4 * i + 2] = r[4 * kPitch];
+      a[4 * i + 3] = r[4 * kPitch + 8];
+    }
+  }
+  NFF_D static void bias_init(float* acc, const float* bias, int q) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q);
+      acc[4 * j + 0] = acc[4 * j + 2] = b.x;
+      acc[4 * j + 1] = acc[4 * j + 3] = b.y;
+    }
+  }
+  NFF_D static void relu(float* acc) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i] = fmaxf(acc[i], 0.0f);
+  }
+
+  NFF_D void run(const float* /* x: read as fragments from the panel */, const float dir[3], float& sdf, float* feat, int tid) {
+    float* col = panel_ + tid;
+    {
+      float shv[kSh];
+      if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], shv); else sh4(dir[0], dir[1], dir[2], shv);
+#pragma unroll
+      for (int i = 0; i < kSh; ++i) col[(kGeoIn + i) * kPitch] = shv[i];
+    }
+    group_sync();  // all 128 panel columns of the group are in
+    const int ln = tid & 31, q = ln & 3;
+    // accumulator fragment (row g (+8), columns 8j + 2q (+1)) of tile row 64h + 16 warp + g: panel column fr + 64 h
+    float* const fr = panel_ + (tid & ~127) + 16 * ((tid >> 5) & 3) + (ln >> 2);
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      float* const p = fr + 64 * h;
+      float a[16], acc[16];
+      // layer 0: grid features -> hidden, ReLU, sdf
+      load_a(a, p, q, 0, 4);
+      bias_init(acc, t->bias[0], q);
+      half_mma<4, 32>(acc, a, t->b + tc_layer_off(0));
+      relu(acc);
+      float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 w = *reinterpret_cast<const float2*>(t->w_sdf + 8 * j + 2 * q);
+        s0 = fmaf(acc[4 * j + 0], w.x, fmaf(acc[4 * j + 1], w.y, s0));
+        s1 = fmaf(acc[4 * j + 2], w.x, fmaf(acc[4 * j + 3], w.y, s1));
+      }
+      s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+      s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+      if (q == 0) {
+        p[(kGeoIn + kSh) * kPitch] = s0 + t->b_sdf;
+        p[(kGeoIn + kSh) * kPitch + 8] = s1 + t->b_sdf;
+      }
+      // layer 1: -> geo_embedding, parked at this thread's fragment positions of panel rows 0..31
+      chain(a, acc);
+      bias_init(acc, t->bias[1], q);
+      half_mma<4, 32>(acc, a, t->b + tc_layer_off(1));
+      __syncwarp();  // the warp's layer-0 fragment loads of these rows are done
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float* r = p + (8 * j + 2 * q) * kPitch;
+        r[0] = acc[4 * j + 0], r[kPitch] = acc[4 * j + 1], r[8] = acc[4 * j + 2], r[kPitch + 8] = acc[4 * j + 3];
+      }
+      // layer 2: [geo_embedding | SH] -> hidden, ReLU
+      chain(a, acc);
+      bias_init(acc, t->bias[2], q);
+      half_mma<4, 48>(acc, a, t->b + tc_layer_off(2));
+      load_a(a, p, q, 4, 2);
+      half_mma<2, 48>(acc, a, t->b + tc_layer_off(2) + 4 * 64);
+      relu(acc);
+      // layer 3: hidden -> hidden, ReLU
+      chain(a, acc);
+      bias_init(acc, t->bias[3], q);
+      half_mma<4, 32>(acc, a, t->b + tc_layer_off(3));
+      relu(acc);
+      // layer 4: hidden -> features, accumulated onto bias + geo_embedding; out to the same positions
+      chain(a, acc);
+      bias_init(acc, t->bias[4], q);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float* r = p + (8 * j + 2 * q) * kPitch;
+        acc[4 * j + 0] += r[0], acc[4 * j + 1] += r[kPitch], acc[4 * j + 2] += r[8], acc[4 * j + 3] += r[kPitch + 8];
+      }
+      half_mma<4, 32>(acc, a, t->b + tc_layer_off(4));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float* r = p + (8 * j + 2 * q) * kPitch;
+        r[0] = acc[4 * j + 0], r[kPitch] = acc[4 * j + 1], r[8] = acc[4 * j + 2], r[kPitch + 8] = acc[4 * j + 3];
+      }
+    }
+    group_sync();  // every tile row's outputs are in
+#pragma unroll
+    for (int i = 0; i < kNff; ++i) feat[i] = col[i * kPitch];
+    sdf = col[(kGeoIn + kSh) * kPitch];
   }
 };
 #endif
@@ -450,7 +586,7 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
     e_prev = e1;
     if (s == kS2 - 1) e1 = fadd(e1, fsub(sp.sky_distance, e1));  // sky sample (neurad.py:451-455)
     Gauss g = sample_gaussian(o, d, area, e0, e1);
-    float* col = mlp.panel() + tid;  // this thread's column of the [32][kLaneThreads] shared panel
+    float* col = mlp.panel() + tid;  // this thread's column of the [32][Mlp::kPitch] shared panel
     float dir[3] = {d[0], d[1], d[2]};
     int aid = -1;
     {
@@ -460,12 +596,12 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
         Gauss ga = {pb[0], pb[1], pb[2], g.std};
         ga = contract(ga, fm.actor_scale);
 #pragma unroll
-        for (int i = 16; i < 32; ++i) col[i * kLaneThreads] = 0.0f;  // F.pad(actor_features, (0, 32-16))
+        for (int i = 16; i < 32; ++i) col[i * Mlp::kPitch] = 0.0f;  // F.pad(actor_features, (0, 32-16))
         if (LAYOUT == 1) {
           const float x4[4] = {ga.x, ga.y, ga.z, fdiv((float)aid, fm.n_actors_f)};
-          tcnn_encode_f4<4>(fm.act, 4, x4, ga.std, col, kLaneThreads);
+          tcnn_encode_f4<4>(fm.act, 4, x4, ga.std, col, Mlp::kPitch);
         } else {
-          encode_f4_col(fm.actor_tables[aid], fm.act, 4, ga, col);
+          encode_f4_col(fm.actor_tables[aid], fm.act, 4, ga, col, Mlp::kPitch);
         }
         float q0 = fadd(fadd(fmul(M[0], d[0]), fmul(M[1], d[1])), fmul(M[2], d[2]));
         float q1 = fadd(fadd(fmul(M[4], d[0]), fmul(M[5], d[1])), fmul(M[6], d[2]));
@@ -476,15 +612,15 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
         Gauss gs = contract(g, fm.static_scale);
         if (LAYOUT == 1) {
           const float x3[3] = {gs.x, gs.y, gs.z};
-          tcnn_encode_f4<3>(fm.stat, 8, x3, gs.std, col, kLaneThreads);
+          tcnn_encode_f4<3>(fm.stat, 8, x3, gs.std, col, Mlp::kPitch);
         } else {
-          encode_f4_col(fm.stat.table, fm.stat, 8, gs, col);
+          encode_f4_col(fm.stat.table, fm.stat, 8, gs, col, Mlp::kPitch);
         }
       }
     }
     float x[kGeoIn];
 #pragma unroll
-    for (int i = 0; i < kGeoIn; ++i) x[i] = col[i * kLaneThreads];
+    for (int i = 0; i < kGeoIn; ++i) x[i] = col[i * Mlp::kPitch];
     float sdf, feat[kNff];
     mlp.run(x, dir, sdf, feat, tid);
     const float alpha = frcp(fadd(1.0f, expf(fmul(sdf, P.beta))));
@@ -535,7 +671,7 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
     // instructions -- to the local buffer and, for the fused multi-GPU gather, to every peer's buffer over NVLink
     // (st.global on peer-mapped addresses; small scattered remote writes are what made the naive version slow).
     const int ln = tid & 31;
-    float* slice = mlp.panel() + (tid & ~31);  // rows 0..31 (stride kLaneThreads) x 32 columns of this warp
+    float* slice = mlp.panel() + (tid & ~31);  // rows 0..11 (stride Mlp::kPitch) x 32 columns of this warp
     const unsigned act_mask = __ballot_sync(0xffffffffu, active);
 #pragma unroll 1
     for (int g = 0; g < 4; ++g) {
@@ -545,12 +681,12 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
 #pragma unroll
         for (int j = 0; j < kNff; ++j) {
           const int slot = r * (kNff + kApp) + j;
-          slice[(slot >> 5) * kLaneThreads + (slot & 31)] = fsum[j];
+          slice[(slot >> 5) * Mlp::kPitch + (slot & 31)] = fsum[j];
         }
 #pragma unroll
         for (int j = 0; j < kApp; ++j) {
           const int slot = r * (kNff + kApp) + kNff + j;
-          slice[(slot >> 5) * kLaneThreads + (slot & 31)] = app[j];
+          slice[(slot >> 5) * Mlp::kPitch + (slot & 31)] = app[j];
         }
       }
       __syncwarp();
@@ -561,7 +697,7 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
       for (int t = 0; t < 3; ++t) {
         const int f = t * 32 + ln;  // float4 index inside the segment's 96 float4
         if (f / 12 < k) {
-          const float4 v = *reinterpret_cast<const float4*>(&slice[(f >> 3) * kLaneThreads + ((f & 7) << 2)]);
+          const float4 v = *reinterpret_cast<const float4*>(&slice[(f >> 3) * Mlp::kPitch + ((f & 7) << 2)]);
           reinterpret_cast<float4*>(P.out.features + ray0 * fdim)[f] = v;
           for (int p = 0; p < P.peers.n_peers; ++p) {
             if (p == P.peers.self_rank) continue;

@@ -130,12 +130,18 @@ __device__ __forceinline__ uint32_t b_elem_offset(int n, int k, int k_pad) {
 }
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
-// cooperative: all `nthreads` threads of the CTA
+// Input column of B row k when the A operand is the previous layer's accumulator fragment taken as is: a thread holds
+// D columns 8j+2t, 8j+2t+1 and the TF32 A fragment wants columns 8j+t, 8j+t+4, so the K rows of each 8-wide chunk are
+// permuted to match (p < 4: column 2p; p >= 4: column 2(p-4)+1).
+__host__ __device__ constexpr int chained_k(int k) { return (k & ~7) | ((k & 7) < 4 ? 2 * (k & 7) : 2 * (k & 7) - 7); }
+
+// cooperative: all `nthreads` threads of the CTA.  The first `k_chained` K rows are permuted by chained_k.
 __device__ __forceinline__ void stage_b_tile(float* hi, float* lo, const float* __restrict__ w, int n_real, int k_real, int n_pad,
-                                             int k_pad, int tid, int nthreads) {
+                                             int k_pad, int tid, int nthreads, int k_chained = 0) {
   for (int i = tid; i < n_pad * k_pad; i += nthreads) {
     int n = i / k_pad, k = i % k_pad;
-    float v = (n < n_real && k < k_real) ? w[n * k_real + k] : 0.0f;
+    const int kw = k < k_chained ? chained_k(k) : k;
+    float v = (n < n_real && kw < k_real) ? w[n * k_real + kw] : 0.0f;
     float h = tf32_hi(v);
     uint32_t off = b_elem_offset(n, k, k_pad);
     hi[off] = h;

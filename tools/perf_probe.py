@@ -10,8 +10,16 @@ if os.environ.get('NFF_LIB'):
 from neurad_studio_b200 import scene
 from neurad_studio_b200.backend import B200Backend
 
-n_actors = int(sys.argv[1]) if len(sys.argv) > 1 else 0
-reps = int(sys.argv[2]) if len(sys.argv) > 2 else 5
+# perf_probe.py [n_actors] [reps] [--profile DIR]: with --profile the timed renders run under torch.profiler (CUDA
+# activities) instead; per-kernel device times go to stdout and DIR/kernels.json, the trace to DIR/render.pt.trace.json
+argv = list(sys.argv[1:])
+prof_dir = None
+if "--profile" in argv:
+    i = argv.index("--profile")
+    prof_dir = argv[i + 1]
+    del argv[i:i + 2]
+n_actors = int(argv[0]) if len(argv) > 0 else 0
+reps = int(argv[1]) if len(argv) > 1 else 5
 be = B200Backend(torch.device("cuda", 0))
 cfg = nsb.NeuRADConfig(n_actors=n_actors)
 trajs = scene.make_trajectories(n_actors, cfg.duration) if n_actors else None
@@ -42,6 +50,26 @@ IW = int(os.environ.get("IMAGE_WIDTH", "0"))
 for _ in range(2):
     be.render(rays, image_width=IW)
 torch.cuda.synchronize()
+if prof_dir:
+    import json
+    from torch.profiler import ProfilerActivity, profile
+
+    os.makedirs(prof_dir, exist_ok=True)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            be.render(rays, image_width=IW)
+        torch.cuda.synchronize()
+    kern = {}
+    for e in prof.key_averages():
+        if e.device_time_total > 0:
+            kern[e.key] = {"calls": e.count, "total_us": e.device_time_total, "mean_us": e.device_time_total / max(e.count, 1)}
+    per_render = sum(v["total_us"] for v in kern.values()) / reps
+    for k, v in sorted(kern.items(), key=lambda kv: -kv[1]["total_us"]):
+        print(f"{v['mean_us'] / 1e3:9.3f} ms x {v['calls']:4d}  {100 * v['total_us'] / reps / per_render:5.1f} %  {k}")
+    json.dump({"rays": N, "reps": reps, "image_width": IW, "device": torch.cuda.get_device_name(), "kernels": kern},
+              open(os.path.join(prof_dir, "kernels.json"), "w"), indent=1)
+    prof.export_chrome_trace(os.path.join(prof_dir, "render.pt.trace.json"))
+    sys.exit(0)
 ts = []
 for _ in range(reps):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
