@@ -309,9 +309,10 @@ int b200nerf_pdf_resample_stratified(b200nerf_ctx* ctx, const float* weights, co
 
 /* ---- backward operators (SURVEY.md 8f, row f2): gradients of the module-level operators with respect to the trained
  * parameters.  The reference gets these from torch autograd (torch mode) or tiny-cuda-nn's backward kernels; here each
- * forward operator has a hand-written counterpart.  Sample positions carry no gradient (PDFSampler detaches its bins,
- * ray_samplers.py:363-364; camera / actor-pose optimisation is not part of this row).  All grad_* outputs are
- * ACCUMULATED into (+=): zero them first (they are the .grad tensors of the parameters). */
+ * forward operator has a hand-written counterpart.  Sample bins carry no gradient (PDFSampler detaches them,
+ * ray_samplers.py:363-364); the sample MEANS do when the camera poses are optimised (b200nerf_neurad_encoding_mean_bwd,
+ * b200nerf_isotropic_gaussian_bwd).  All grad_* outputs are ACCUMULATED into (+=): zero them first (they are the .grad
+ * tensors of the parameters); the d* outputs of the two position-gradient operators are written. */
 
 /* Backward of b200nerf_neurad_encoding_fwd for field `field`: scatter-add into the hash-table gradients.
  *   features mode: dfeatures [N*S, L*F] = dL/d features.
@@ -336,6 +337,32 @@ int b200nerf_neurad_encoding_pose_bwd(b200nerf_ctx* ctx, int field, const float*
                                       const float* flip, int64_t n_rays, int n_samples, const float* dfeatures,
                                       const float* rotations_6d, const float* positions, float* grad_rotations_6d,
                                       float* grad_positions, void* stream);
+
+/* Gradient of b200nerf_neurad_encoding_fwd (features or density output) with respect to the sample MEANS, for camera
+ * pose optimisation (CameraOptimizer.apply_to_raybundle, cameras/camera_optimizers.py:173-182): dmean [N,S,3] is
+ * WRITTEN (one row per sample, no accumulation).  Mode selection as b200nerf_neurad_encoding_bwd: dfeatures [N*S, L*F]
+ * (features mode, F = 4), or density [N,S] + ddensity [N,S] (density mode, F = 1, through trunc_exp and the density
+ * decoder, fields/neurad_field.py:208-213).  Per sample the gradient combines
+ *   - the static lookup through ScaledSceneContraction(order=inf) (field_components/spatial_distortions.py:103-114,
+ *     132-136): the contracted mean and, outside the unit cube, the std scaling that changes the anti-aliasing level
+ *     weights 1 / max(1, 2 res std) (neurad_encoding.py:297-304); at a tie of |x_i| the inf-norm's gradient is split
+ *     evenly, as torch's backward does;
+ *   - for a sample inside an actor box, the actor lookup chained through the box transform and the training-mode x
+ *     flip (neurad_encoding.py:174-219) -- only for field B200NERF_FIELD_MAIN, whose grid the reference builds with
+ *     require_actor_grad (fields/neurad_field.py:50).  In the proposal fields the actor branch runs under no_grad and
+ *     overwrites the static features, so an actor sample's dmean is exactly 0.
+ * Directions carry no gradient (the SH encoding is no_grad in torch mode, encodings.py:797-800).  An empty batch is a
+ * no-op. */
+int b200nerf_neurad_encoding_mean_bwd(b200nerf_ctx* ctx, int field, const float* mean, const float* std, const float* times,
+                                      const float* flip, int64_t n_rays, int n_samples, const float* dfeatures,
+                                      const float* density, const float* ddensity, float* dmean, void* stream);
+
+/* Frustums.get_fast_isotropic_gaussian backward (cameras/rays.py:109-124): mean_s = o + d t_s with t_s = start_s +
+ * (end_s - start_s) / 2 of the euclidean edges bins_e [N,S+1] (the same t as b200nerf_isotropic_gaussian_fwd; the bins
+ * are detached, std does not depend on o or d).  dmean [N,S,3] -> dorigins = sum_s dmean_s and ddirections =
+ * sum_s t_s dmean_s, both [N,3], WRITTEN.  An empty batch is a no-op. */
+int b200nerf_isotropic_gaussian_bwd(b200nerf_ctx* ctx, const float* bins_e, int64_t n_rays, int n_samples, const float* dmean,
+                                    float* dorigins, float* ddirections, void* stream);
 
 /* HashEncoding.forward backward (autograd of encodings.py:425-466 / tcnn's grid backward) for the stand-alone grid operator
  * b200nerf_hashgrid_fwd: x [P,3], dout [P, L*F] -> grad_table [L*T, F] accumulated (+=).  L*F <= 64. */

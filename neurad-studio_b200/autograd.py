@@ -4,10 +4,12 @@ mirror (NeuRADField / NeuRADProposalField / RaySamples.get_weights / renderers, 
 the hash tables, density decoders, MLPs and beta without any torch reference math in between.
 
 The reference gets these gradients from torch autograd (implementation="torch") or tiny-cuda-nn's backward kernels
-(field_components/encodings.py:386-404, mlp.py:116-140).  Sample positions carry no gradient (PDFSampler detaches its
-bins, ray_samplers.py:363-364); the actor trajectories do, through the main field's box-frame positions
+(field_components/encodings.py:386-404, mlp.py:116-140).  Sample bins carry no gradient (PDFSampler detaches them,
+ray_samplers.py:363-364); the actor trajectories do, through the main field's box-frame positions
 (require_actor_grad, neurad_encoding.py:174; EncodingFn); the box-frame directions do not (torch-mode SHEncoding is
-no_grad, encodings.py:797-800); camera optimisation is off in NeuRAD's config."""
+no_grad, encodings.py:797-800).  With a camera optimizer the ray origins and directions require grad: the sample means
+then receive a gradient from EncodingFn / DensityFn, and IsotropicGaussianFn passes it on to the rays
+(cameras/camera_optimizers.py:173-182, cameras/rays.py:109-124)."""
 from __future__ import annotations
 
 from typing import List, Optional
@@ -23,9 +25,10 @@ _bwd = torch.amp.custom_bwd(device_type="cuda")
 
 
 class EncodingFn(Function):
-    """NeuRADHashEncoding.forward: (features [N*S,D], directions [N,S,3]); gradients go to the hash tables and -- for a
-    field built with require_actor_grad (the main field, fields/neurad_field.py:50) -- to the actor trajectories
-    `actor_rotations_6d` [T,A,6] / `actor_positions` [T,A,3] (pass None for a field without trajectory gradients)."""
+    """NeuRADHashEncoding.forward: (features [N*S,D], directions [N,S,3]); gradients go to the hash tables, the sample
+    means (when they require grad: camera optimisation) and -- for a field built with require_actor_grad (the main
+    field, fields/neurad_field.py:50) -- to the actor trajectories `actor_rotations_6d` [T,A,6] / `actor_positions`
+    [T,A,3] (pass None for a field without trajectory gradients)."""
 
     @staticmethod
     @_fwd
@@ -55,11 +58,15 @@ class EncodingFn(Function):
         if rot6 is not None and pos is not None and (ctx.needs_input_grad[7] or ctx.needs_input_grad[8]):
             g_rot, g_pos = torch.zeros_like(rot6), torch.zeros_like(pos)
             ctx.be.neurad_encoding_pose_bwd(ctx.field, mean, std, times, dfeatures, rot6, pos, g_rot, g_pos, flip=flip)
-        return (None,) * 7 + (g_rot if ctx.needs_input_grad[7] else None, g_pos if ctx.needs_input_grad[8] else None, g_static, *g_actors)
+        g_mean = None
+        if ctx.needs_input_grad[2]:
+            g_mean = ctx.be.neurad_encoding_mean_bwd(ctx.field, mean, std, times, dfeatures=dfeatures, flip=flip).reshape(mean.shape)
+        return (None, None, g_mean) + (None,) * 4 + (g_rot if ctx.needs_input_grad[7] else None, g_pos if ctx.needs_input_grad[8] else None, g_static, *g_actors)
 
 
 class DensityFn(Function):
-    """NeuRADProposalField.get_density: density [N,S]; gradients go to the hash tables and the density decoder."""
+    """NeuRADProposalField.get_density: density [N,S]; gradients go to the hash tables, the density decoder and (when
+    they require grad: camera optimisation) the sample means."""
 
     @staticmethod
     @_fwd
@@ -91,7 +98,34 @@ class DensityFn(Function):
         if g_static is not None or any(t is not None for t in g_actors):
             ctx.be.neurad_encoding_bwd(ctx.field, mean, std, times, {"static": g_static, "actors": g_actors, "decoder": None},
                                        density=density, ddensity=ddensity, flip=flip)
-        return (None,) * 6 + (g_static, g_dec, *g_actors)
+        g_mean = None
+        if ctx.needs_input_grad[2]:
+            g_mean = ctx.be.neurad_encoding_mean_bwd(ctx.field, mean, std, times, density=density, ddensity=ddensity,
+                                                     flip=flip).reshape(mean.shape)
+        return (None, None, g_mean) + (None,) * 3 + (g_static, g_dec, *g_actors)
+
+
+class IsotropicGaussianFn(Function):
+    """Frustums.get_fast_isotropic_gaussian (cameras/rays.py:109-124): (mean [N,S,3], std [N,S]); gradients go to the
+    per-ray origins and directions [N,3] through the mean (the bins are detached; std depends on neither)."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, be, origins, directions, pixel_area, bins_e):
+        mean, std = be.isotropic_gaussian(origins, directions, pixel_area, bins_e)
+        ctx.be = be
+        ctx.shapes = (origins.shape, directions.shape)
+        ctx.save_for_backward(bins_e)
+        ctx.mark_non_differentiable(std)
+        return mean, std
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, dmean, _dstd):
+        (bins_e,) = ctx.saved_tensors
+        do, dd = ctx.be.isotropic_gaussian_bwd(bins_e, dmean.contiguous())
+        return (None, do.reshape(ctx.shapes[0]) if ctx.needs_input_grad[1] else None,
+                dd.reshape(ctx.shapes[1]) if ctx.needs_input_grad[2] else None, None, None)
 
 
 class MlpFn(Function):
@@ -268,7 +302,8 @@ class InterlevelLossFn(Function):
 
 class HashGridFn(Function):
     """HashEncoding.forward (the stand-alone grid, encodings.py:425-471): gradient to the hash table (the reference also
-    differentiates with respect to the positions; the path never asks for that on a stand-alone grid)."""
+    differentiates with respect to the positions; NeuRAD's path never asks for that on a stand-alone grid -- its position
+    gradients go through NeuRADHashEncoding: EncodingFn / DensityFn)."""
 
     @staticmethod
     @_fwd

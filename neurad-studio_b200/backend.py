@@ -562,6 +562,38 @@ class B200Backend:
         self._check(self.lib.b200nerf_neurad_encoding_pose_bwd(self._h, field, _ptr(m), _ptr(sd), _ptr(t), _ptr(fl), n, s, _ptr(df), _ptr(r6),
                                                                _ptr(ps), _ptr(grad_rotations_6d), _ptr(grad_positions), self._stream))
 
+    def neurad_encoding_mean_bwd(self, field: int, mean: torch.Tensor, std: torch.Tensor, times: Optional[torch.Tensor],
+                                 dfeatures: Optional[torch.Tensor] = None, density: Optional[torch.Tensor] = None,
+                                 ddensity: Optional[torch.Tensor] = None, flip: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """dL/d mean [N,S,3] of neurad_encoding (features mode: dfeatures; density mode: density + ddensity), for camera
+        pose optimisation.  Actor samples contribute for the main field only (require_actor_grad); a proposal field's
+        actor samples get exactly 0."""
+        if (dfeatures is None) == (ddensity is None) or (ddensity is not None and density is None):
+            raise ValueError("pass either dfeatures or (density, ddensity)")
+        m = self._dev(mean)
+        n, s = m.shape[0], m.shape[1]
+        m = m.reshape(n, s, 3)
+        sd = self._dev(std).reshape(n, s)
+        t = self._ray_times(times, n)
+        fl = None if flip is None else self._dev(flip).reshape(n)
+        df = None if dfeatures is None else self._dev(dfeatures).reshape(n * s, dfeatures.shape[-1])
+        de = None if density is None else self._dev(density).reshape(n, s)
+        dd = None if ddensity is None else self._dev(ddensity).reshape(n, s)
+        dmean = torch.empty(n, s, 3, device=self.device)
+        self._check(self.lib.b200nerf_neurad_encoding_mean_bwd(self._h, field, _ptr(m), _ptr(sd), _ptr(t), _ptr(fl), n, s, _ptr(df), _ptr(de),
+                                                               _ptr(dd), _ptr(dmean), self._stream))
+        return dmean
+
+    def isotropic_gaussian_bwd(self, bins_e: torch.Tensor, dmean: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Backward of isotropic_gaussian: euclidean edges [N,S+1], dmean [N,S,3] -> (d origins [N,3], d directions [N,3])."""
+        b = self._dev(bins_e)
+        n, s = b.shape[0], b.shape[1] - 1
+        dm = self._dev(dmean).reshape(n, s, 3)
+        do = torch.empty(n, 3, device=self.device)
+        dd = torch.empty(n, 3, device=self.device)
+        self._check(self.lib.b200nerf_isotropic_gaussian_bwd(self._h, _ptr(b), n, s, _ptr(dm), _ptr(do), _ptr(dd), self._stream))
+        return do, dd
+
     def hashgrid_bwd(self, g: HashGridSettings, x: torch.Tensor, dout: torch.Tensor, grad_table: torch.Tensor,
                      scalings: Optional[torch.Tensor] = None) -> None:
         """Backward of hashgrid_fwd: accumulates dL/d hash_table [L*T,F] from dL/d out [P, L*F]."""

@@ -3,13 +3,15 @@
 Mirrors the subset of the reference's config tree that shapes ``NeuRADModel.get_nff_outputs``:
 ``NeuRADModelConfig`` / ``SamplingSettings`` (nerfstudio/models/neurad.py:97-162), ``NeuRADFieldConfig`` /
 ``NeuRADProposalFieldConfig`` (nerfstudio/fields/neurad_field.py:44-75, 155-182) and ``StaticSettings`` /
-``ActorSettings`` (nerfstudio/field_components/neurad_encoding.py:34-66).  Field names follow the reference.
+``ActorSettings`` (nerfstudio/field_components/neurad_encoding.py:34-66), and the camera pose optimizer's
+``CameraOptimizerConfig`` / ``ScaledCameraOptimizerConfig`` (nerfstudio/cameras/camera_optimizers.py:43-60,335-357).
+Field names follow the reference.
 """
 from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Tuple
+from typing import Tuple, Union
 
 import numpy as np
 import torch
@@ -122,6 +124,36 @@ class NeuRADConfig:
     @property
     def feature_dim(self) -> int:
         return self.nff_out_dim + self.appearance_dim
+
+
+@dataclass
+class CameraOptimizerConfig:
+    """Camera pose optimisation (cameras/camera_optimizers.py:43-60): "off" (NeuRAD's default, models/neurad.py), or a
+    per-camera 6-vector [translation | rotation] mapped to a pose correction by exp_map_SO3xR3 / exp_map_SE3
+    (cameras/lie_groups.py).  The penalties weight the L2 norms of the two halves in get_loss_dict."""
+
+    mode: str = "off"  # "off" | "SO3xR3" | "SE3"
+    trans_l2_penalty: Union[Tuple[float, ...], float] = 1e-2
+    rot_l2_penalty: float = 1e-3
+
+    def __post_init__(self):
+        if self.mode not in ("off", "SO3xR3", "SE3"):
+            raise ValueError(f"camera optimizer mode must be 'off', 'SO3xR3' or 'SE3', not {self.mode!r}")
+
+
+@dataclass
+class ScaledCameraOptimizerConfig(CameraOptimizerConfig):
+    """Axis-weighted pose optimisation (camera_optimizers.py:335-357): the 6-vector is multiplied by `weights` before the
+    exp map; the translation penalty is per axis and applied to |t| (an L1 term).  neurad-scaleopt and its siblings
+    (configs/method_configs.py:438-495) use mode "SO3xR3" with weights (1, 1, 0.01, 0.01, 0.01, 1)."""
+
+    weights: Tuple[float, float, float, float, float, float] = (1.0, 1.0, 1.0, 1.0, 1.0, 1.0)
+    trans_l2_penalty: Union[Tuple[float, float, float], float] = (1e-2, 1e-2, 1e-2)
+
+
+def scaleopt_camera_optimizer() -> ScaledCameraOptimizerConfig:
+    """The camera optimizer of neurad-scaleopt / neurader-scaleopt / neuradest-scaleopt (method_configs.py:440-442)."""
+    return ScaledCameraOptimizerConfig(mode="SO3xR3", weights=(1.0, 1.0, 0.01, 0.01, 0.01, 1.0))
 
 
 def small_config(n_actors: int = 0, log2_main: int = 12, log2_prop: int = 11, **kw) -> NeuRADConfig:

@@ -1701,6 +1701,46 @@ int b200nerf_neurad_encoding_pose_bwd(b200nerf_ctx* c, int field, const float* m
   return 0;
 }
 
+int b200nerf_neurad_encoding_mean_bwd(b200nerf_ctx* c, int field, const float* mean, const float* std, const float* times,
+                                      const float* flip, int64_t n_rays, int n_samples, const float* dfeatures,
+                                      const float* density, const float* ddensity, float* dmean, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(field >= 0 && field < 3, "field must be B200NERF_FIELD_MAIN / PROP0 / PROP1");
+  if (!c->have_field[field]) return fail(B200NERF_ERR_STATE, "b200nerf_set_field_grids was not called for this field");
+  REQUIRE(n_rays >= 0 && n_samples >= 1, "bad sample grid");
+  // as in b200nerf_neurad_encoding_bwd: an empty batch's tensors may be NULL, every other check holds for it too
+  const bool empty = n_rays == 0;
+  REQUIRE(!(dfeatures && ddensity), "pass either dfeatures or (density, ddensity)");
+  REQUIRE(empty || dfeatures || ddensity, "pass either dfeatures or (density, ddensity)");
+  REQUIRE(empty || !ddensity || density, "density mode needs the forward density");
+  const FieldGrids& fg = c->fields[field];
+  if (ddensity && !fg.decoder) return fail(B200NERF_ERR_STATE, "b200nerf_set_proposal_decoder was not called for this field");
+  if (c->actors.n_actors > kModMaxActors) return fail(B200NERF_ERR_UNSUPPORTED, "more than 64 actors");
+  if (empty) return 0;
+  REQUIRE(mean && std && dmean, "NULL argument");
+  REQUIRE(c->actors.n_actors == 0 || times, "times are required when the scene has actors");
+  DeviceGuard g(c->device);
+  // require_actor_grad: the main field's grid only (fields/neurad_field.py:50,177)
+  MeanBwdArgs a{mean, std, times, flip, dfeatures, density, ddensity, dmean, n_rays, n_samples, field == B200NERF_FIELD_MAIN ? 1 : 0};
+  if (!launch_neurad_encoding_mean_bwd(fg, c->actors, a, (cudaStream_t)stream))
+    return fail(B200NERF_ERR_UNSUPPORTED, "encoding mean backward: features mode needs 4 features / level, density mode 1 (<= 8 levels)");
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b200nerf_isotropic_gaussian_bwd(b200nerf_ctx* c, const float* bins_e, int64_t n_rays, int n_samples, const float* dmean,
+                                    float* dorigins, float* ddirections, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n_rays >= 0 && n_samples >= 1, "bad sample grid");
+  if (n_rays == 0) return 0;
+  REQUIRE(bins_e && dmean && dorigins && ddirections, "NULL argument");
+  DeviceGuard g(c->device);
+  const unsigned grid = (unsigned)((n_rays + kModWarps - 1) / kModWarps);
+  isotropic_gaussian_bwd_kernel<<<grid, kModWarps * 32, 0, (cudaStream_t)stream>>>(bins_e, dmean, n_rays, n_samples, dorigins, ddirections);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 int b200nerf_hashgrid_bwd(b200nerf_ctx* c, const b200nerf_grid_desc* desc, const float* x, const float* dout, int64_t n_points,
                           float* grad_table, void* stream) {
   REQUIRE(c, "ctx is NULL");

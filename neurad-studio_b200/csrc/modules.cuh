@@ -655,6 +655,105 @@ __global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_pose_bwd_kerne
   }
 }
 
+// Gradient of NeuRADHashEncoding.forward (or NeuRADProposalField.get_density) with respect to the sample means, for
+// camera pose optimisation: dmean [N,S,3], written with plain stores (each sample owns its row, no atomics).  The
+// thread mapping is the forward's (neurad_encoding_fwd_kernel): one warp per ray builds the ray's actor frames in shared
+// memory once, then lane = sample.  The scatter backward's segment-per-thread walk exists to run-length aggregate
+// REDUCTIONS into shared table rows; here there is nothing to aggregate, and lane = sample makes the mean / std / dmean
+// accesses of a warp contiguous.  MODE 1: features (F = 4), MODE 2: density (F = 1).
+struct MeanBwdArgs {
+  const float* mean;       // [N,S,3]
+  const float* std;        // [N,S]
+  const float* times;      // [N]
+  const float* flip;       // [N] or NULL
+  const float* dfeatures;  // [N*S, D]  (features mode)
+  const float* density;    // [N,S]     (density mode: forward output)
+  const float* ddensity;   // [N,S]     (density mode)
+  float* dmean;            // [N,S,3]   written
+  int64_t n_rays;
+  int32_t S, actor_grad;
+};
+template <int MODE>
+__global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_mean_bwd_kernel(const FieldGrids fg, const Actors A, const MeanBwdArgs a) {
+  static_assert(MODE == 1 || MODE == 2, "features or density mode");
+  constexpr int F = MODE == 1 ? 4 : 1;
+  extern __shared__ __align__(16) unsigned char mean_bwd_smem[];
+  const int warp = threadIdx.x >> 5, ln = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * kModWarps + warp;
+  if (ray >= a.n_rays) return;
+  ActorFrame* frames = reinterpret_cast<ActorFrame*>(mean_bwd_smem) + warp * A.n_actors;
+  if (A.n_actors > 0) {
+    int left, right;
+    float frac;
+    keyframe_bracket(A, a.times[ray], left, right, frac);
+    for (int k = ln; k < A.n_actors; k += 32) actor_frame(A, k, left, right, frac, frames[k]);
+  }
+  __syncwarp();
+  const int D = fg.stat.L * fg.stat.F;
+  const float flip = a.flip ? a.flip[ray] : 1.0f;
+  for (int s = ln; s < a.S; s += 32) {
+    const int64_t i = ray * a.S + s;
+    const Gauss g = {a.mean[3 * i], a.mean[3 * i + 1], a.mean[3 * i + 2], a.std[i]};
+    float gp[3];
+    if (MODE == 1) {
+      neurad_encode_point_mean_bwd_t<F>(fg, frames, A.n_actors, a.actor_grad != 0, g, flip, a.dfeatures + i * D, 1.0f, gp);
+    } else {
+      // trunc_exp backward (field_components/activations.py:38-41), as in encoding_bwd_segment_pending
+      const float gd = a.ddensity[i] * fminf(fmaxf(a.density[i], 3.0590232e-07f), 3269017.372f);
+      neurad_encode_point_mean_bwd_t<F>(fg, frames, A.n_actors, a.actor_grad != 0, g, flip, fg.decoder, gd, gp);
+    }
+    a.dmean[3 * i] = gp[0];
+    a.dmean[3 * i + 1] = gp[1];
+    a.dmean[3 * i + 2] = gp[2];
+  }
+}
+inline bool launch_neurad_encoding_mean_bwd(const FieldGrids& fg, const Actors& A, const MeanBwdArgs& a, cudaStream_t stream) {
+  const unsigned grid = (unsigned)((a.n_rays + kModWarps - 1) / kModWarps);
+  if (grid == 0) return true;
+  // 64 B per actor and warp: 32 KB at kModMaxActors, under the 48 KB default
+  const size_t smem = sizeof(ActorFrame) * kModWarps * (size_t)A.n_actors;
+  if (!a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 4))
+    neurad_encoding_mean_bwd_kernel<1><<<grid, kModWarps * 32, smem, stream>>>(fg, A, a);
+  else if (a.ddensity && encode_bwd_fast_ok(fg, A.n_actors, 1))
+    neurad_encoding_mean_bwd_kernel<2><<<grid, kModWarps * 32, smem, stream>>>(fg, A, a);
+  else
+    return false;
+  return true;
+}
+
+// Frustums.get_fast_isotropic_gaussian backward (cameras/rays.py:109-124): dmean [N,S,3] -> d origins [N,3],
+// d directions [N,3] (written).  One warp per ray, lane = sample (coalesced dmean reads), then a warp sum.
+__global__ void __launch_bounds__(kModWarps * 32) isotropic_gaussian_bwd_kernel(const float* __restrict__ bins_e, const float* __restrict__ dmean,
+                                                                                int64_t n_rays, int S, float* __restrict__ dorigins,
+                                                                                float* __restrict__ ddirs) {
+  const int warp = threadIdx.x >> 5, ln = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * kModWarps + warp;
+  if (ray >= n_rays) return;
+  float go[3] = {0.f, 0.f, 0.f}, gd[3] = {0.f, 0.f, 0.f};
+  for (int s = ln; s < S; s += 32) {
+    const int64_t i = ray * S + s;
+    const float t = gaussian_t(bins_e[ray * (S + 1) + s], bins_e[ray * (S + 1) + s + 1]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float g = dmean[3 * i + k];
+      go[k] += g;
+      gd[k] = fmaf(t, g, gd[k]);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    go[k] = warp_sum(go[k]);
+    gd[k] = warp_sum(gd[k]);
+  }
+  if (ln == 0) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      dorigins[3 * ray + k] = go[k];
+      ddirs[3 * ray + k] = gd[k];
+    }
+  }
+}
+
 // HashEncoding.forward backward (the stand-alone grid of field_components/encodings.py:425-466, no anti-aliasing rescale):
 // grad_table[row] += dout[p, l*F+f] * trilinear corner weight; one thread per point.
 __global__ void hashgrid_bwd_kernel(Grid g, const float* __restrict__ x, const float* __restrict__ dout, int64_t n_points,

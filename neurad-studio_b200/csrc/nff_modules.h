@@ -685,6 +685,126 @@ NFF_D int neurad_encode_point_pose_bwd(const FieldGrids& fg, const Actors& A, co
   return a;
 }
 
+// ------------------------------------------------------------------------------ gradients to the sample positions
+// Camera pose optimisation (cameras/camera_optimizers.py:173-182) moves the ray origins and directions, so the sample
+// means (cameras/rays.py:109-124) carry a gradient through the hash-grid lookups.  Per sample and lookup:
+//   u = contract(p), features_lf = trilerp_lf(u * res_l) * w_l(std_u)   (encodings.py:425-466, neurad_encoding.py:297-304)
+// The std depends on p only through the contraction's std scaling (spatial_distortions.py:132-136), which changes the
+// level weights w_l = 1 / max(1, 2 res_l std_u) where 2 res_l std_u >= 1 (torch's clamp_min passes the gradient at the
+// bound): d w_l / d std_u = -2 res_l w_l^2.
+//
+// One contracted lookup: g_u = dL/du (the position term of encode_levels_pos_grad, with 16-byte row loads for F = 4)
+// and g_s = dL/d std_u.  src / scale as in encode_levels_bwd_t (features mode: the dfeatures row, scale 1; density mode:
+// the decoder weights, scale = dL/d density * trunc_exp').  WANT_STD = false skips the level-weight term (the caller
+// knows the std does not depend on p).
+template <int LMAX, int F, bool WANT_STD>
+NFF_D void encode_levels_mean_grad_t(const float* NFF_RESTRICT table, const Grid& gr, const Gauss& g, const float* NFF_RESTRICT src,
+                                     float scale, float gu[3], float& gs) {
+  static_assert(F == 1 || F == 4, "NeuRAD's feature widths");
+  gu[0] = gu[1] = gu[2] = 0.0f;
+  gs = 0.0f;
+#pragma unroll
+  for (int l = 0; l < LMAX; ++l) {
+    if (l < gr.L) {
+      const float res = gr.res[l];
+      const Cell c = grid_cell(g.x, g.y, g.z, res);
+      uint32_t r[8];
+      cell_rows(c, gr.mask, r);
+      const float w = level_weight(res, g.std);
+      const float* base = table + (size_t)l * gr.T * F;
+      float v[F][8], df[F];
+      if (F == 4) {
+        const float4 d4 = ldg(reinterpret_cast<const float4*>(src) + l);
+        df[0] = scale * d4.x, df[F > 1 ? 1 : 0] = scale * d4.y, df[F > 2 ? 2 : 0] = scale * d4.z, df[F > 3 ? 3 : 0] = scale * d4.w;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float4 q = ldg(reinterpret_cast<const float4*>(base) + r[k]);
+          v[0][k] = q.x, v[F > 1 ? 1 : 0][k] = q.y, v[F > 2 ? 2 : 0][k] = q.z, v[F > 3 ? 3 : 0][k] = q.w;
+        }
+      } else {
+        df[0] = scale * ldg(src + l);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[0][k] = ldg(base + r[k]);
+      }
+      const float wr = w * res;
+      const bool clamped = WANT_STD && fmul(fmul(res, 2.0f), g.std) >= 1.0f;
+      float acc_v = 0.0f;
+#pragma unroll
+      for (int f = 0; f < F; ++f) {
+        float dt[3];
+        trilerp_grad(v[f], c, dt);
+        const float s = df[f] * wr;
+        gu[0] = fmaf(s, dt[0], gu[0]);
+        gu[1] = fmaf(s, dt[1], gu[1]);
+        gu[2] = fmaf(s, dt[2], gu[2]);
+        if (clamped) acc_v = fmaf(df[f], trilerp(v[f], c), acc_v);
+      }
+      if (clamped) gs = fmaf(acc_v, -2.0f * res * w * w, gs);
+    }
+  }
+}
+
+// Backward of contract() (ScaledSceneContraction(order=inf), spatial_distortions.py:103-114,132-136) for one gaussian:
+// dL/du (contracted position) and dL/d std_u -> dL/dp.  x = p / scale, m = |x|_inf; outside the unit cube
+// y = (2 - 1/m) x / m and std_u = std / scale * ((2m - 1)^(1/3) / m)^2 / 4, both functions of m.  At a tie of |x_i|
+// the gradient of m is split evenly between the tied coordinates, as torch's backward of the inf-norm does
+// (linalg_vector_norm_backward: sign(x) * mask / mask.sum()).
+NFF_D void contract_bwd(const Gauss& g, float scale, const float gu[3], float gs, float gp[3]) {
+  const float inv = frcp(scale);
+  const float x[3] = {fdiv(g.x, scale), fdiv(g.y, scale), fdiv(g.z, scale)};
+  const float m = fmaxf(fmaxf(fabsf(x[0]), fabsf(x[1])), fabsf(x[2]));
+  const float gy[3] = {0.25f * gu[0], 0.25f * gu[1], 0.25f * gu[2]};
+  if (m < 1.0f) {
+    for (int i = 0; i < 3; ++i) gp[i] = gy[i] * inv;
+    return;
+  }
+  const float im = 1.0f / m, a = 2.0f - im;
+  // d/dm [(2 - 1/m) / m] = 2 (1 - m) / m^3;  d/dm [(2m - 1)^(2/3) / m^2] = (4/3) (2m - 1)^(-1/3) / m^2 - 2 (2m - 1)^(2/3) / m^3
+  const float da = 2.0f * (1.0f - m) * im * im * im;
+  const float c = cbrtf(2.0f * m - 1.0f);
+  const float dq2 = (4.0f / 3.0f) / c * im * im - 2.0f * c * c * im * im * im;
+  float gm = da * (gy[0] * x[0] + gy[1] * x[1] + gy[2] * x[2]) + 0.25f * gs * g.std * inv * dq2;
+  const int ties = (fabsf(x[0]) == m) + (fabsf(x[1]) == m) + (fabsf(x[2]) == m);
+  gm /= (float)ties;
+  for (int i = 0; i < 3; ++i) {
+    float gx = gy[i] * a * im;
+    if (fabsf(x[i]) == m) gx += x[i] < 0.0f ? -gm : gm;
+    gp[i] = gx * inv;
+  }
+}
+
+// dL/d mean of one sample of field `fg` (NeuRADHashEncoding.forward, neurad_encoding.py:150-187): the static lookup
+// through the contraction, or -- for a sample inside an actor box -- the actor lookup through its contraction, the
+// training-mode x flip and the world -> box transform q = B^T (p - t) (neurad_encoding.py:174-219).  `actor_grad`
+// is the reference's require_actor_grad (fields/neurad_field.py:50,177): for the proposal fields the actor branch runs
+// under no_grad and its rows overwrite the static features (index_put), so an actor sample's gradient is exactly 0.
+template <int F>
+NFF_D void neurad_encode_point_mean_bwd_t(const FieldGrids& fg, const ActorFrame* frames, int n_actors, bool actor_grad, const Gauss& g,
+                                          float flip, const float* src, float scale, float gp[3]) {
+  gp[0] = gp[1] = gp[2] = 0.0f;
+  float pb[3];
+  const int a = n_actors > 0 ? actor_containing(frames, n_actors, g.x, g.y, g.z, pb) : -1;
+  float gu[3], gs;
+  if (a >= 0) {
+    if (!actor_grad) return;
+    const Gauss ga = {flip < 0.0f ? -pb[0] : pb[0], pb[1], pb[2], g.std};
+    encode_levels_mean_grad_t<8, F, true>(fg.actor_tables[a], fg.act, contract(ga, fg.actor_scale), src, scale, gu, gs);
+    float gq[3];
+    contract_bwd(ga, fg.actor_scale, gu, gs, gq);
+    if (flip < 0.0f) gq[0] = -gq[0];
+    const float* M = frames[a].w2b;  // q_i = sum_j M[4i + j] p_j + M[4i + 3]
+    for (int j = 0; j < 3; ++j) gp[j] = M[j] * gq[0] + M[4 + j] * gq[1] + M[8 + j] * gq[2];
+    return;
+  }
+  encode_levels_mean_grad_t<8, F, true>(fg.stat.table, fg.stat, contract(g, fg.static_scale), src, scale, gu, gs);
+  contract_bwd(g, fg.static_scale, gu, gs, gp);
+}
+
+// Frustums.get_fast_isotropic_gaussian backward for one ray (cameras/rays.py:109-124): mean_s = o + d t_s with
+// t_s = start_s + (end_s - start_s) / 2 of the detached bins (exactly sample_gaussian's t); std_s does not depend on
+// o or d.  d o += dmean_s, d d += t_s dmean_s.
+NFF_D float gaussian_t(float start, float end) { return fadd(start, fdiv(fsub(end, start), 2.0f)); }
+
 // ------------------------------------------------------------------------------------------------ training losses
 // The two per-ray regularisers NeuRAD trains with (models/neurad.py:262,524,541-545), one thread per ray; both are
 // functions of the `weights_list` / `ray_samples_list` the module walk returns.

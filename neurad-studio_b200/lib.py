@@ -123,6 +123,9 @@ SIGNATURES = {
                                              c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_void_p]),
     "b200nerf_neurad_encoding_pose_bwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p,
                                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200nerf_neurad_encoding_mean_bwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200nerf_isotropic_gaussian_bwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200nerf_hashgrid_bwd": (c_int, [c_void_p, POINTER(GridDesc), c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "b200nerf_alpha_to_weights_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "b200nerf_density_to_weights_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),

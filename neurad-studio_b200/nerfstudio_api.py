@@ -13,6 +13,7 @@ modules, so that the parity tests read like the reference's own tests and a refe
   model_components/ray_samplers.py:56,135,838  Spaced/Uniform/.../PowerSampler  same names (-> spaced_sample kernel)
   cameras/rays.py:33,127        Frustums, RaySamples           same names (get_positions / get_weights kernels)
   model_components/renderers.py:59,93,322,353  Feature/RGB/Accumulation/DepthRenderer  same names (-> composite kernel)
+  cameras/camera_optimizers.py:84,359  CameraOptimizer, ScaledCameraOptimizer  same names (exp maps in torch on [C,6])
   models/neurad.py:165          NeuRADModel.get_nff_outputs /  NeuRADModel       (-> fused nff_render_fwd kernel)
                                 get_outputs_for_camera_ray_bundle / decode_features (lidar half)
   field_components/neurad_encoding.py:85  NeuRADHashEncoding   NeuRADHashEncoding (-> neurad_encoding_fwd kernel)
@@ -39,7 +40,7 @@ from torch import Tensor, nn
 
 from . import autograd as AG
 from .backend import B200Backend
-from .config import HashGridSettings, NeuRADConfig
+from .config import CameraOptimizerConfig, HashGridSettings, NeuRADConfig, ScaledCameraOptimizerConfig
 
 _BACKENDS: Dict[int, B200Backend] = {}
 _UIDS = itertools.count(1)  # one token per model instance (id() can be reused after garbage collection)
@@ -376,14 +377,17 @@ class Frustums:
         be = get_backend(self.bin_edges.device)
         return be.frustum_positions(self.origins, self.directions, self.bin_edges, normalize_aabb)
 
-    @torch.no_grad()
     def get_fast_isotropic_gaussian(self, num_multisamples: int = 1) -> GaussiansStd:
-        """rays.py:109-124 (NeuRAD uses one multisample, neurad_field.py:67)."""
+        """rays.py:109-124 (NeuRAD uses one multisample, neurad_field.py:67).  Differentiable with respect to the origins
+        and directions when they require grad (camera pose optimisation); the bins are detached as in the reference."""
         if num_multisamples != 1:
             raise NotImplementedError("num_multisamples != 1")
         assert self.pixel_area is not None, "frustums built without pixel_area"
         be = get_backend(self.bin_edges.device)
-        return GaussiansStd(*be.isotropic_gaussian(self.origins, self.directions, self.pixel_area, self.bin_edges))
+        if _needs_grad(self.origins, self.directions):
+            return GaussiansStd(*AG.IsotropicGaussianFn.apply(be, self.origins, self.directions, self.pixel_area, self.bin_edges.detach()))
+        with torch.no_grad():
+            return GaussiansStd(*be.isotropic_gaussian(self.origins, self.directions, self.pixel_area, self.bin_edges))
 
 
 @dataclass
@@ -472,7 +476,11 @@ class SpacedSampler:
             bins_s, bins_e = be.spaced_sample(ray_bundle.nears, ray_bundle.fars, n, self.spacing, lam, scaling)
         area = None if ray_bundle.pixel_area is None else ray_bundle.pixel_area.reshape(-1, 1)
         times = None if ray_bundle.times is None else ray_bundle.times.reshape(-1, 1)
-        return RaySamples(Frustums(ray_bundle.origins.reshape(-1, 3), ray_bundle.directions.reshape(-1, 3), bins_e, area), bins_s,
+        # (a view taken under no_grad does not carry the bundle's autograd history: keep [N,3] tensors as they are, so
+        # that corrected origins / directions of a camera optimizer stay differentiable)
+        o, d = ray_bundle.origins, ray_bundle.directions
+        o, d = (o if o.dim() == 2 else o.reshape(-1, 3)), (d if d.dim() == 2 else d.reshape(-1, 3))
+        return RaySamples(Frustums(o, d, bins_e, area), bins_s,
                           times=times, metadata=ray_bundle.metadata,
                           spacing=(self.spacing, lam, scaling, ray_bundle.nears, ray_bundle.fars))
 
@@ -685,7 +693,8 @@ class NeuRADHashEncoding:
 
     def forward(self, positions: GaussiansStd, times: Tensor, directions: Optional[Tensor] = None) -> Tuple[Tensor, Optional[Tensor]]:
         """(features [N*S, D], directions [N,S,3] in the actor frame where a sample is inside an actor | None); trains the
-        tables (and, for the main field's grid, the actor trajectories) when they require grad."""
+        tables (and, for the main field's grid, the actor trajectories) when they require grad, and passes a gradient to
+        positions.mean when it requires one (camera pose optimisation)."""
         m = self._model
         be = m._bind()
         flip = m._draw_actor_flip(positions.mean.shape[0], self._field)
@@ -693,7 +702,7 @@ class NeuRADHashEncoding:
         traj = [None, None]
         if self._field == 0 and m.config.n_actors:  # require_actor_grad: the main field's grid only (neurad_field.py:50,177)
             traj = [m._param("dynamic_actors.actor_rotations_6d"), m._param("dynamic_actors.actor_positions")]
-        if _needs_grad(*tables, *traj):
+        if _needs_grad(*tables, *traj, positions.mean):
             feats, dirs = AG.EncodingFn.apply(be, self._field, positions.mean, positions.std, times, directions, flip, traj[0], traj[1],
                                               tables[0], *tables[1:])
             return feats, (dirs if directions is not None else None)
@@ -713,7 +722,8 @@ class NeuRADProposalField:
 
     def get_density(self, ray_samples: RaySamples) -> Tuple[Tensor, None]:
         """density [N,S,1] = trunc_exp(density_decoder(hashgrid(gaussians))) (neurad_field.py:208-213); with grad mode
-        on and trainable parameters the backward operator delivers d/d(hash tables, density_decoder.weight)."""
+        on and trainable parameters the backward operator delivers d/d(hash tables, density_decoder.weight), and d/d mean
+        when the frustums' origins / directions require grad (camera pose optimisation)."""
         m = self._model
         pos = ray_samples.frustums.get_fast_isotropic_gaussian(num_multisamples=1)
         be = m._bind()
@@ -721,7 +731,7 @@ class NeuRADProposalField:
         pre = f"proposal_fields.{self._field - 1}"
         tables = m._grid_params(pre)
         dec = m._param(f"{pre}.density_decoder.weight")
-        if torch.is_grad_enabled() and any(t.requires_grad for t in tables + [dec]):
+        if _needs_grad(*tables, dec, pos.mean):
             dens = AG.DensityFn.apply(be, self._field, pos.mean, pos.std, ray_samples.times, flip, tables[0], dec, *tables[1:])
             return dens[..., None], None
         with torch.no_grad():
@@ -741,8 +751,9 @@ class NeuRADField:
         self.hashgrid = NeuRADHashEncoding(model, 0)
 
     def forward(self, ray_samples: RaySamples, compute_normals: bool = False) -> Dict[FieldHeadNames, Tensor]:
-        """{FEATURE [N,S,32], SDF [N,S,1], ALPHA [N,S,1]}.  With grad mode on and trainable parameters every stage is an
-        autograd node with a hand-written backward operator (hash tables, both MLPs, beta)."""
+        """{FEATURE [N,S,32], SDF [N,S,1], ALPHA [N,S,1]}.  With grad mode on and trainable parameters (or sample means
+        that require grad) every stage is an autograd node with a hand-written backward operator (hash tables, both MLPs,
+        beta, sample means)."""
         if compute_normals:
             raise NotImplementedError("NeuRADField never computes normals (neurad_field.py:128)")
         m = self._model
@@ -756,7 +767,7 @@ class NeuRADField:
         beta = m._param("field.sdf_to_density.beta")
         # the main field's grid has require_actor_grad (neurad_field.py:50): its features also train the trajectories
         traj = [m._param("dynamic_actors.actor_rotations_6d"), m._param("dynamic_actors.actor_positions")] if m.config.n_actors else [None, None]
-        if torch.is_grad_enabled() and any(t.requires_grad for t in tables + geo_wb + feat_wb + [beta] + [t for t in traj if t is not None]):
+        if _needs_grad(*tables, *geo_wb, *feat_wb, beta, *traj, g.mean):
             feats, dirs = AG.EncodingFn.apply(be, 0, g.mean, g.std, ray_samples.times, ray_samples.frustums.directions, flip,
                                               traj[0], traj[1], tables[0], *tables[1:])
             geo = AG.MlpFn.apply(be, feats, *geo_wb)
@@ -840,6 +851,155 @@ class RGBDecoder(nn.Sequential):
         return be.rgb_decode(features, impl)
 
 
+def _skew(v: Tensor) -> Tensor:
+    """[C,3] -> the cross-product matrices [C,3,3] ([v]x w = v x w)."""
+    z = torch.zeros_like(v[:, 0])
+    return torch.stack([torch.stack([z, -v[:, 2], v[:, 1]], -1), torch.stack([v[:, 2], z, -v[:, 0]], -1),
+                        torch.stack([-v[:, 1], v[:, 0], z], -1)], -2)
+
+
+def exp_map_SO3xR3(tangent: Tensor) -> Tensor:
+    """cameras/lie_groups.py exp_map_SO3xR3: [C,6] = (translation, rotation vector) -> [C,3,4].  The rotation is Rodrigues'
+    formula R = I + sin(a)/a K + (1 - cos(a))/a^2 K^2 with K = [w]x and a = |w|; like the reference, a is taken as
+    sqrt(max(|w|^2, 1e-4)) inside the two coefficients (K itself is not clamped); the translation is used as is."""
+    w = tangent[:, 3:]
+    a = (w * w).sum(dim=1).clamp(min=1e-4).sqrt()
+    k = _skew(w)
+    eye = torch.eye(3, dtype=tangent.dtype, device=tangent.device)
+    rot = eye + (a.sin() / a)[:, None, None] * k + ((1.0 - a.cos()) / (a * a))[:, None, None] * (k @ k)
+    return torch.cat([rot, tangent[:, :3, None]], dim=-1)
+
+
+def exp_map_SE3(tangent: Tensor) -> Tensor:
+    """cameras/lie_groups.py exp_map_SE3: [C,6] = (rho, rotation vector w) -> [C,3,4] = [R | V rho] with
+    R = I + A K + B K^2, V = I + B K + C K^2, A = sin(a)/a, B = (1 - cos a)/a^2, C = (a - sin a)/a^3 (K = [w]x, a = |w|).
+    Below a = 1e-2 the coefficients are their Taylor series (the reference switches at the same angle; the two differ by
+    O(a^4) there)."""
+    rho, w = tangent[:, :3], tangent[:, 3:]
+    a = w.norm(dim=1)
+    small = a < 1e-2
+    a2 = a * a
+    a_nz = torch.where(small, torch.ones_like(a), a)
+    ca = torch.where(small, 1.0 - a2 / 6.0, a_nz.sin() / a_nz)
+    cb = torch.where(small, 0.5 - a2 / 24.0, (1.0 - a_nz.cos()) / (a_nz * a_nz))
+    cc = torch.where(small, 1.0 / 6.0 - a2 / 120.0, (a_nz - a_nz.sin()) / (a_nz * a_nz * a_nz))
+    k = _skew(w)
+    k2 = k @ k
+    eye = torch.eye(3, dtype=tangent.dtype, device=tangent.device)
+    rot = eye + ca[:, None, None] * k + cb[:, None, None] * k2
+    v = eye + cb[:, None, None] * k + cc[:, None, None] * k2
+    return torch.cat([rot, v @ rho[:, :, None]], dim=-1)
+
+
+class CameraOptimizer(nn.Module):
+    """cameras/camera_optimizers.py:84-233: per-camera pose corrections.  With mode "SO3xR3" / "SE3" the parameter
+    `pose_adjustment` [num_cameras, 6] (translation | rotation, zero-initialised) maps through the exp map to [R | t];
+    `apply_to_raybundle` then sets o' = o + t and d' = R d (not renormalised).  With mode "off" the module holds nothing.
+
+    `non_trainable_camera_indices`: like the reference, forward() sets the correction ROWS at these positions of its
+    output to the identity -- rows of the `indices` batch, not rows whose camera index matches (the two agree for
+    get_correction_matrices(), whose batch is every camera in order)."""
+
+    def __init__(self, config: CameraOptimizerConfig, num_cameras: int, device="cpu",
+                 non_trainable_camera_indices: Optional[Tensor] = None, **kwargs) -> None:
+        super().__init__()
+        self.config = config
+        self.num_cameras = num_cameras
+        self.device = device
+        self.non_trainable_camera_indices = non_trainable_camera_indices
+        if config.mode != "off":
+            self.pose_adjustment = nn.Parameter(torch.zeros((num_cameras, 6), device=device))
+
+    def _get_pose_adjustment(self) -> Tensor:
+        return self.pose_adjustment
+
+    def forward(self, indices: Tensor) -> Tensor:
+        """Correction matrices [len(indices), 3, 4] (identity with mode "off")."""
+        if self.config.mode == "off":
+            return torch.eye(4, device=indices.device)[None, :3, :4].tile(indices.shape[0], 1, 1)
+        adj = self._get_pose_adjustment()[indices, :]
+        out = exp_map_SO3xR3(adj) if self.config.mode == "SO3xR3" else exp_map_SE3(adj)
+        if self.non_trainable_camera_indices is not None:
+            idx = self.non_trainable_camera_indices.to(out.device)
+            self.non_trainable_camera_indices = idx
+            out[idx] = torch.eye(4, device=out.device)[:3, :4]
+        return out
+
+    def apply_to_raybundle(self, raybundle: RayBundle) -> None:
+        """Corrects the flattened bundle in place (camera_optimizers.py:173-182): origins += t, directions = R d."""
+        if self.config.mode == "off":
+            return
+        corr = self(raybundle.camera_indices.squeeze())
+        raybundle.origins = raybundle.origins + corr[:, :3, 3]
+        raybundle.directions = torch.bmm(corr[:, :3, :3], raybundle.directions[..., None]).squeeze().to(raybundle.origins)
+
+    def apply_to_camera(self, camera) -> Tensor:
+        """camera_optimizers.py:184-207: the corrected sensor-to-world [C,3,4] of a Cameras / Lidars object whose
+        metadata names its camera (`cam_idx`); the rotation multiplies from the left, the translation is added."""
+        s2w = camera.camera_to_worlds if hasattr(camera, "camera_to_worlds") else camera.lidar_to_worlds
+        md = getattr(camera, "metadata", None)
+        if self.config.mode == "off" or md is None or "cam_idx" not in md:
+            return s2w
+        adj = self(torch.tensor([md["cam_idx"]], dtype=torch.long, device=s2w.device))
+        return torch.cat([torch.bmm(adj[..., :3, :3], s2w[..., :3, :3]), s2w[..., :3, 3:] + adj[..., :3, 3:]], dim=-1)
+
+    def get_loss_dict(self, loss_dict: dict) -> None:
+        """camera_opt_regularizer = mean |t| * trans_l2_penalty + mean |w| * rot_l2_penalty (:209-216)."""
+        if self.config.mode != "off":
+            adj = self._get_pose_adjustment()
+            loss_dict["camera_opt_regularizer"] = (adj[:, :3].norm(dim=-1).mean() * self.config.trans_l2_penalty
+                                                   + adj[:, 3:].norm(dim=-1).mean() * self.config.rot_l2_penalty)
+
+    def get_correction_matrices(self) -> Tensor:
+        return self(torch.arange(0, self.num_cameras).long())
+
+    def get_metrics_dict(self, metrics_dict: dict) -> None:
+        """Translation max / mean and rotation mean / max in degrees (:222-230)."""
+        if self.config.mode != "off":
+            trans = self.pose_adjustment[:, :3].detach().norm(dim=-1)
+            rot = self.pose_adjustment[:, 3:].detach().norm(dim=-1)
+            metrics_dict["camera_opt_translation_max"] = trans.max()
+            metrics_dict["camera_opt_translation_mean"] = trans.mean()
+            metrics_dict["camera_opt_rotation_mean"] = torch.rad2deg(rot.mean().cpu())
+            metrics_dict["camera_opt_rotation_max"] = torch.rad2deg(rot.max().cpu())
+
+    def get_param_groups(self, param_groups: dict) -> None:
+        params = list(self.parameters())
+        if self.config.mode != "off":
+            assert len(params) > 0
+            param_groups["camera_opt"] = params
+        else:
+            assert len(params) == 0
+
+
+class ScaledCameraOptimizer(CameraOptimizer):
+    """camera_optimizers.py:359-383: the pose adjustment is multiplied by the `weights` buffer before the exp map and the
+    regulariser; the translation penalty is per axis on |t|."""
+
+    def __init__(self, config: ScaledCameraOptimizerConfig, **kwargs) -> None:
+        super().__init__(config, **kwargs)
+        self.register_buffer("weights", torch.tensor(config.weights, dtype=torch.float32))
+        self.trans_penalty = torch.tensor(config.trans_l2_penalty, dtype=torch.float32, device=self.device)
+
+    def _get_pose_adjustment(self) -> Tensor:
+        return self.pose_adjustment * self.weights
+
+    def get_loss_dict(self, loss_dict: dict) -> None:
+        if self.config.mode != "off":
+            adj = self._get_pose_adjustment()
+            self.trans_penalty = self.trans_penalty.to(adj.device)
+            loss_dict["camera_opt_regularizer"] = ((adj[:, :3].abs() * self.trans_penalty).mean()
+                                                   + adj[:, 3:].norm(dim=-1).mean() * self.config.rot_l2_penalty)
+
+
+def make_camera_optimizer(config: Optional[CameraOptimizerConfig], num_cameras: int, device="cpu",
+                          non_trainable_camera_indices: Optional[Tensor] = None) -> CameraOptimizer:
+    """CameraOptimizerConfig.setup(): the scaled variant for a ScaledCameraOptimizerConfig."""
+    config = CameraOptimizerConfig() if config is None else config
+    cls = ScaledCameraOptimizer if isinstance(config, ScaledCameraOptimizerConfig) else CameraOptimizer
+    return cls(config=config, num_cameras=num_cameras, device=device, non_trainable_camera_indices=non_trainable_camera_indices)
+
+
 class NeuRADModel(nn.Module):
     """models/neurad.py:165 with the reference's parameter names: `state_dict()` / `load_state_dict()` speak the reference's
     dotted keys (`field.hashgrid.static_grid.hash_table`, ...; a `_model.` prefix as in `checkpoint["pipeline"]` is accepted),
@@ -850,11 +1010,16 @@ class NeuRADModel(nn.Module):
     `get_nff_outputs` is ONE fused kernel launch (ray sampling, both proposal rounds, main field, compositing); the
     reference's 32 768-ray chunk loop (neurad.py:650-659) is unnecessary because nothing per-sample goes to HBM."""
 
-    def __init__(self, config: NeuRADConfig, trajectories: Optional[List[dict]] = None, implementation: str = "torch") -> None:
+    def __init__(self, config: NeuRADConfig, trajectories: Optional[List[dict]] = None, implementation: str = "torch",
+                 camera_optimizer: Optional[CameraOptimizerConfig] = None, num_cameras: int = 1, use_camopt_in_eval: bool = False,
+                 non_trainable_camera_indices: Optional[Tensor] = None) -> None:
         """`implementation`: which of the reference's two parameter layouts the model holds (models/neurad.py:146) --
         "torch" (per-level hashed tables, nn.Linear MLPs; trainable here) or "tcnn" (the reference's default: flat
         `tcnn_encoding.params` vectors in tiny-cuda-nn's layout, so that a tcnn-trained checkpoint loads with
-        `load_state_dict`; inference through the fused kernels only -- SURVEY 8f row f3, tcnn_compat.py)."""
+        `load_state_dict`; inference through the fused kernels only -- SURVEY 8f row f3, tcnn_compat.py).
+
+        `camera_optimizer` / `use_camopt_in_eval`: ADModelConfig's fields (models/ad_model.py:40-45); None = mode "off".
+        `num_cameras` sizes `camera_optimizer.pose_adjustment` (the reference's num_train_data)."""
         super().__init__()
         from . import scene  # synthetic init = the reference's random init shapes
 
@@ -899,6 +1064,9 @@ class NeuRADModel(nn.Module):
         self.density_fns = [lambda ray_samples: last.get_density(ray_samples)[0] for _ in self.proposal_fields]
         self.renderer_feat = FeatureRenderer()
         self.renderer_accumulation = AccumulationRenderer()
+        # ad_model.py:70-72; state dict keys camera_optimizer.pose_adjustment (+ .weights) as in the reference
+        self.camera_optimizer = make_camera_optimizer(camera_optimizer, num_cameras, non_trainable_camera_indices=non_trainable_camera_indices)
+        self.use_camopt_in_eval = use_camopt_in_eval
 
     # -- nn.Module state dict in the reference's key format --------------------------------------------------------
     @staticmethod
@@ -922,10 +1090,12 @@ class NeuRADModel(nn.Module):
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
         """nn.Module.load_state_dict on the reference's keys.  Even with strict=False a missing tensor of THIS path (grids,
         MLPs, decoders, appearance embedding, actor trajectories) raises: silently keeping a random init is never wanted.
-        The rgb decoder stays optional in a hot-path-only state dict; keys of other subsystems are ignored when not strict."""
+        The rgb decoder stays optional in a hot-path-only state dict; keys of other subsystems are ignored when not strict.
+        With a camera optimizer that is on, `camera_optimizer.pose_adjustment` (and `.weights`) are required too."""
         res = super().load_state_dict(dict(state_dict), strict=strict, assign=assign)
         back = {n: k for n, k in self._names}
-        missing = [back[k] for k in res.missing_keys if k in back]
+        # a camera optimizer that is on needs its pose corrections (mode "off" has no tensors, as in the reference)
+        missing = [back.get(k, k) for k in res.missing_keys if k in back or k.startswith("camera_optimizer.")]
         if missing:
             raise KeyError(f"state dict lacks hot-path tensors: {missing[:6]}{' ...' if len(missing) > 6 else ''}")
         return res
@@ -945,12 +1115,18 @@ class NeuRADModel(nn.Module):
     def load_reference_state_dict(self, sd: Dict[str, Tensor]) -> None:
         """Copy tensors from a reference `NeuRADModel.state_dict()` (keys like
         `field.hashgrid.static_grid.hash_table`, `proposal_fields.1.density_decoder.weight`); unknown keys (rgb
-        decoder, camera optimizer, losses) are ignored, missing hot-path keys raise."""
+        decoder, losses) are ignored, missing hot-path keys raise; the camera optimizer's tensors are required when its
+        mode is not "off" and ignored otherwise."""
         for n, k in self._names:
             if k not in sd:
                 raise KeyError(f"reference state dict lacks {k}")
             with torch.no_grad():  # in place on the tensor itself (not .data): bumps _version, which _bind() watches
                 getattr(self, n).copy_(sd[k].to(getattr(self, n).dtype))
+        for k, t in self.camera_optimizer.state_dict(keep_vars=True).items():
+            if "camera_optimizer." + k not in sd:
+                raise KeyError(f"reference state dict lacks camera_optimizer.{k}")
+            with torch.no_grad():
+                t.copy_(sd["camera_optimizer." + k].to(t.dtype))
         dec = {k[len("rgb_decoder."):]: v for k, v in sd.items() if k.startswith("rgb_decoder.")}
         if dec:  # the camera decoder is optional in a hot-path-only state dict
             self.rgb_decoder.load_state_dict(dec, strict=False)
@@ -978,8 +1154,10 @@ class NeuRADModel(nn.Module):
         the library -- the per-module API of SURVEY 8b; additionally returns the reference's training-side extras
         `weights_list` / `ray_samples_list` (neurad.py:404-405)."""
         # only the parameters of THIS path count (the rgb decoder's nn.Conv2d weights require grad by default, but it is
-        # evaluated after this function and is inference-only)
-        wants_grad = torch.is_grad_enabled() and any(getattr(self, n).requires_grad for n, _ in self._names)
+        # evaluated after this function and is inference-only); camera_optimizer.pose_adjustment counts through the
+        # bundle: a bundle corrected by a trainable camera optimizer has origins / directions that require grad
+        wants_grad = torch.is_grad_enabled() and (any(getattr(self, n).requires_grad for n, _ in self._names)
+                                                  or _needs_grad(ray_bundle.origins, ray_bundle.directions))
         if self.implementation == "tcnn" and (wants_grad or fused is False):
             raise NotImplementedError("tiny-cuda-nn-layout parameters render through the fused kernels only (inference of "
                                       "tcnn-trained checkpoints); the module walk and training use the torch layout")
@@ -1182,8 +1360,12 @@ class NeuRADModel(nn.Module):
 
     def get_outputs(self, ray_bundle: RayBundle, patch_size: Tuple[int, int], intensity_for_cam: bool = False,
                     calc_lidar_losses: bool = True) -> Dict[str, Tensor]:
-        """neurad.py:311-335: get_nff_outputs + decode_features; `features` is dropped from the result.  (The camera
-        optimizer's `apply_to_raybundle` of training mode is pose optimisation: not part of this path.)"""
+        """neurad.py:311-335: in training mode (or with use_camopt_in_eval) the camera optimizer corrects the flattened
+        bundle first (:318-319; a no-op with mode "off"), then get_nff_outputs + decode_features; `features` is dropped
+        from the result."""
+        if (self.training or self.use_camopt_in_eval) and self.camera_optimizer.config.mode != "off":
+            ray_bundle = ray_bundle.flatten()
+            self.camera_optimizer.apply_to_raybundle(ray_bundle)
         out = self.get_nff_outputs(ray_bundle, calc_lidar_losses)
         rgb, intensity, ray_drop_logits = self.decode_features(out["features"], patch_size, ray_bundle.flatten().metadata.get("is_lidar"),
                                                                intensity_for_cam)
@@ -1215,8 +1397,14 @@ class NeuRADModel(nn.Module):
 
     @torch.no_grad()
     def get_outputs_for_camera_ray_bundle(self, camera_ray_bundle: RayBundle) -> Dict[str, Tensor]:
-        """neurad.py:623-675: 2-D bundles are subsampled at
-        [step//2::step] like the reference (`compensate_upsampling_when_rendering`), 1-D bundles are lidar rays."""
+        """neurad.py:623-675: in training mode or with use_camopt_in_eval the camera optimizer corrects the bundle first
+        (:630-634), and the fused render takes the corrected rays; 2-D bundles are subsampled at [step//2::step] like the
+        reference (`compensate_upsampling_when_rendering`), 1-D bundles are lidar rays."""
+        if (self.training or self.use_camopt_in_eval) and self.camera_optimizer.config.mode != "off":
+            shape = camera_ray_bundle.shape
+            camera_ray_bundle = camera_ray_bundle.flatten()
+            self.camera_optimizer.apply_to_raybundle(camera_ray_bundle)
+            camera_ray_bundle = camera_ray_bundle._map(lambda t: t.reshape(*shape, t.shape[-1]))
         if len(camera_ray_bundle.shape) == 1:
             output_size = (camera_ray_bundle.shape[0],)
         else:
