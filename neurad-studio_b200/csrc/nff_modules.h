@@ -487,9 +487,10 @@ NFF_D int neurad_encode_point_bwd(const FieldGrids& fg, float* grad_static, floa
 }
 
 // nerfacc.render_weight_from_alpha backward for one ray (sequential; S <= a few hundred): w_i = a_i * T_i,
-// T_i = prod_{j<i} (1 - a_j)  =>  dL/da_i = dw_i * T_i - (sum_{k>i} dw_k * w_k) / (1 - a_i).
-// The quotient is guarded like nerfacc's backward (1 - a clamped from below) so a saturated sample gives a finite
-// gradient.
+// T_i = prod_{j<i} (1 - a_j)  =>  dL/da_i = T_i * (dw_i - R_i),  R_i = sum_{k>i} dw_k a_k prod_{i<j<k} (1 - a_j),
+// with the suffix recurrence R_{S-1} = 0, R_{i-1} = dw_i a_i + (1 - a_i) R_i.  No division: at a_i == 1 exactly the
+// later samples' weights are 0 but R_i is not, and the result equals autograd of the cumprod (torch's cumprod backward
+// is exact at a zero factor), where dividing sum_{k>i} dw_k w_k by 1 - a_i would lose the occlusion term.
 NFF_D void alpha_weights_bwd_ray(const float* alpha, const float* dw, int S, float* dalpha) {
   float T = 1.0f;
   // forward pass for the transmittances, stored in dalpha[] temporarily
@@ -497,12 +498,11 @@ NFF_D void alpha_weights_bwd_ray(const float* alpha, const float* dw, int S, flo
     dalpha[i] = T;
     T *= 1.0f - alpha[i];
   }
-  float suffix = 0.0f;  // sum_{k>i} dw_k * w_k
+  float R = 0.0f;
   for (int i = S - 1; i >= 0; --i) {
-    const float Ti = dalpha[i];
-    const float one_m = fmaxf(1.0f - alpha[i], 1e-10f);
-    dalpha[i] = dw[i] * Ti - suffix / one_m;
-    suffix += dw[i] * alpha[i] * Ti;
+    const float a = alpha[i];
+    dalpha[i] = dalpha[i] * (dw[i] - R);
+    R = dw[i] * a + (1.0f - a) * R;
   }
 }
 
