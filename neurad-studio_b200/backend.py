@@ -226,7 +226,11 @@ class B200Backend:
         sensor_idx (int64), is_lidar (bool/uint8).  Returns features [N,48], depth/accumulation/prop_depth_i [N,1].
         `out` may supply pre-allocated output tensors (e.g. a slice of an all-gather buffer).  `image_width` > 0
         declares the bundle a row-major image (stack) of that width so that the kernel can walk it in 2-D tiles
-        (better gather coherence); it does not change the output order."""
+        (better gather coherence); it does not change the output order.
+
+        `want_trace`: True records every per-sample trace field (TRACE_FIELDS) next to the outputs; a collection of
+        trace names records only those.  Tracing actor ids turns off the proposal rounds' early exit, so a trace
+        without them is how the production path itself is observed."""
         cfg = self.cfg
         if cfg is None:
             raise RuntimeError("load_params() must be called before render()")
@@ -271,7 +275,14 @@ class B200Backend:
         oo.intensity = res["intensity"].data_ptr() if want_intensity else None
         oo.ray_drop_logit = res["ray_drop_logits"].data_ptr() if want_intensity else None
         tr = None
-        if want_trace:
+        if isinstance(want_trace, (bool, int)) or getattr(want_trace, "dtype", None) == bool:  # incl. numpy / torch bools
+            traced = set(TRACE_FIELDS) if want_trace else set()
+        else:
+            traced = set(want_trace)
+            unknown = traced - set(TRACE_FIELDS)
+            if unknown:
+                raise ValueError(f"unknown trace fields {sorted(unknown)}; known: {list(TRACE_FIELDS)}")
+        if traced:
             S0, S1 = cfg.sampling.num_proposal_samples
             S2 = cfg.sampling.num_nerf_samples
             f32, i32 = torch.float32, torch.int32
@@ -286,6 +297,9 @@ class B200Backend:
             }
             tr = Trace()
             for k in TRACE_FIELDS:
+                if k not in traced:
+                    setattr(tr, k, None)
+                    continue
                 shp, dt = tshapes[k]
                 res[k] = torch.empty(shp, device=self.device, dtype=dt)
                 setattr(tr, k, res[k].data_ptr())
