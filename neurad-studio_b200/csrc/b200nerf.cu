@@ -200,19 +200,29 @@ __device__ __forceinline__ bool lane_patch_ray(const RenderParams& P, int64_t pa
   return lane_unit_ray(P, patch / kPatchesPerUnit, (int)(patch % kPatchesPerUnit) * 32 + lane_, ray_out);
 }
 
-// Two-stage variant of the ray-per-lane path.  Stage 1 (sampling: both proposal rounds) needs no shared memory and fits
-// 64 registers, so it runs at 32 warps/SM with the SM's whole 256 KB L1/shared array as L1; stage 2 (main field + MLPs +
+// Two-stage variant of the ray-per-lane path.  Stage 1 (sampling: both proposal rounds) needs no shared memory beyond round
+// 0's 516 B edge table and fits 64 registers, so it runs at 32 warps/SM with nearly the whole 256 KB L1/shared array as L1; stage 2 (main field + MLPs +
 // compositing) is the tensor-core kernel at 16 warps/SM.  The hand-over is 33 spacing edges per ray ([edge][ray],
 // 132 B/ray) -- still nothing per-sample in HBM.
 #ifndef NFF_SAMPLE_CTAS
 #define NFF_SAMPLE_CTAS 2
 #endif
-template <int LAYOUT>  // 0: the reference's torch-mode grids; 1: tiny-cuda-nn layout (tcnn-trained checkpoints, SURVEY 8f f3)
+// LAYOUT 0: the reference's torch-mode grids; 1: tiny-cuda-nn layout (tcnn-trained checkpoints, SURVEY 8f f3).  ACTORS /
+// TRACED = false leave the actor path / the trace stores out of the code: the untraced instances fit 64 registers without
+// spilling (sample_lane_kernel picks the instance).
+template <int LAYOUT, bool ACTORS, bool TRACED>
 __global__ void __launch_bounds__(kLaneThreads, NFF_SAMPLE_CTAS) nff_sample_lane_kernel(const __grid_constant__ RenderParams P,
                                                                                         float* __restrict__ scratch,
                                                                                         float* __restrict__ handoff) {
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane_ = tid & 31;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
+  // round 0's euclidean edges, when no ray has its own near / far
+  __shared__ float e0_tab[kS0 + 1];
+  const bool shared_edges = !P.rays.nears && !P.rays.fars;
+  if (shared_edges) {
+    if (tid <= kS0) e0_tab[tid] = lane_round0_edge(P.samp, tid);
+    __syncthreads();
+  }
   constexpr int kPPU = kLaneThreads / 32;  // patches per tile
   const int64_t n_patches = lane_patches(P);
   // full rounds: tile k * gridDim + blockIdx (the resident CTAs sweep over ADJACENT tiles together: their working set of
@@ -231,11 +241,20 @@ __global__ void __launch_bounds__(kLaneThreads, NFF_SAMPLE_CTAS) nff_sample_lane
     }
     int64_t ray;
     const bool active = lane_patch_ray(P, patch, lane_, &ray);
-    const LaneRay R = lane_ray_setup(P, sc, tid, ray);
+    const LaneRay R = lane_ray_setup<ACTORS>(P, sc, tid, ray);
     // inactive lanes write their (discarded) edges into the slab column instead of another ray's hand-over column
     float* col = active ? handoff + ray : sc.bins2 + tid;
-    sample_ray_lane<LAYOUT>(P, sc, R, tid, ray, active, col, active ? P.n_rays : (int64_t)kLaneThreads);
+    sample_ray_lane<LAYOUT, ACTORS, TRACED>(P, sc, R, tid, ray, active, col, active ? P.n_rays : (int64_t)kLaneThreads,
+                                            shared_edges ? e0_tab : nullptr);
   }
+}
+// the instance of a launch: `actors` = the scene has actors, `traced` = a proposal-stage trace is recorded (traced renders
+// take the instance with the actor path compiled in)
+template <int LAYOUT>
+static auto sample_lane_kernel(bool actors, bool traced) {
+  return traced ? nff_sample_lane_kernel<LAYOUT, true, true>
+         : actors ? nff_sample_lane_kernel<LAYOUT, true, false>
+                  : nff_sample_lane_kernel<LAYOUT, false, false>;
 }
 
 template <int LAYOUT>
@@ -1031,8 +1050,11 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
                                 (int)lane_tc_smem_bytes()));
   CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 (int)lane_tc_smem_bytes()));
-  CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<0>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));  // all L1
-  CUDA_TRY(cudaFuncSetAttribute(nff_sample_lane_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+  // (almost) all L1: the smallest carve-out that holds the 516 B edge table of each resident CTA
+  for (int i = 0; i < 4; ++i) {
+    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<0>(i & 1, i & 2), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<1>(i & 1, i & 2), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+  }
   CUDA_TRY(cudaMalloc((void**)&c->d_minmax, 2 * sizeof(unsigned)));
   c->handoff_rays = (int64_t)1 << 21;
   CUDA_TRY(cudaMalloc((void**)&c->d_handoff, sizeof(float) * (kS2 + 1) * c->handoff_rays));
@@ -1376,6 +1398,9 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
     // sampling kernel -> [33][rays] spacing edges -> shading kernel; bundles larger than the hand-over buffer are
     // rendered in slices (whole 16-row tile bands when an image_width hint is given)
     const size_t smem = lane_tc_smem_bytes();
+    const b200nerf_trace& tr = P.trace;  // any proposal-stage trace pointer selects the traced sampling kernel
+    const bool traced = tr.prop_weights_0 || tr.prop_weights_1 || tr.actor_id_0 || tr.actor_id_1 || tr.bins_s_1 ||
+                        tr.bins_s_2 || tr.bins_e_1 || tr.bins_e_2 || tr.inds_1 || tr.inds_2;
     int64_t slice = c->handoff_rays;
     if (rays->image_width > 0) {
       const int64_t band = (int64_t)rays->image_width * (kLaneThreads / 32);
@@ -1398,11 +1423,12 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       const int64_t max_a = (int64_t)c->sm_count * NFF_SAMPLE_CTAS, max_b = (int64_t)c->sm_count * kLaneCtasPerSm;
       const int64_t patches = rays->image_width > 0 ? need * (kLaneThreads / 32) : (cnt + 31) / 32, groups = (patches + 3) / 4;
       const int64_t grid_a = patches < max_a ? patches : max_a, grid_b = groups < max_b ? groups : max_b;
+      const bool actors = c->actors.n_actors > 0;
       if (c->layout == 1) {
-        nff_sample_lane_kernel<1><<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        sample_lane_kernel<1>(actors, traced)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
         nff_shade_lane_kernel<1><<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
       } else {
-        nff_sample_lane_kernel<0><<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        sample_lane_kernel<0>(actors, traced)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
         nff_shade_lane_kernel<0><<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
       }
     }

@@ -81,6 +81,12 @@ NFF_D float spacing_fn(float x, const Sampling& s) {
   return fmul(s.ratio, fsub(pow_lam(t, s.lam), 1.0f));
 }
 NFF_D float spacing_fn_inv(float y, const Sampling& s) {
+  if (s.lam == -1.0f) {
+    // NeuRAD's power_lambda, same values as the general path: lam_1 == 2, so (y * -1) / 2 is exactly y * -0.5 (one
+    // rounding of the same real number), and t**-1 is the reciprocal; the division by `scaling` stays IEEE
+    const float t = fmaxf(fadd(fmul(y, -0.5f), 1.0f), 1e-10f);
+    return fdiv(fmul(fsub(frcp(t), 1.0f), s.lam_1), s.scaling);
+  }
   float t = fadd(fdiv(fmul(y, s.lam), s.lam_1), 1.0f);
   t = fmaxf(t, 1e-10f);
   float r = fmul(fsub(pow_lam(t, s.lam == -1.0f ? -1.0f : 1.0f / s.lam), 1.0f), s.lam_1);

@@ -134,11 +134,12 @@ NFF_D int lane_actor_of_sample(const LaneScratch& sc, int tid, int n_cand, const
 }
 
 // LAYOUT 0: the reference's torch layout (hashed [L*T,F] tables, one 3-D grid per actor); 1: tiny-cuda-nn layout (nff_device.h)
-template <int LAYOUT = 0>
+// ACTORS = false: the scene has no actors (n_cand == 0), the actor path is not compiled in.
+template <int LAYOUT = 0, bool ACTORS = true>
 NFF_D float lane_proposal_density(const FieldGrids& fg, const LaneScratch& sc, int tid, int n_cand, const Gauss& g,
                                   int* actor_id) {
   float pb[3], M[12];
-  int a = n_cand > 0 ? lane_actor_of_sample(sc, tid, n_cand, g, pb, M) : -1;
+  int a = ACTORS && n_cand > 0 ? lane_actor_of_sample(sc, tid, n_cand, g, pb, M) : -1;
   float acc;
   if (a >= 0) {
     Gauss ga = {pb[0], pb[1], pb[2], g.std};
@@ -229,18 +230,21 @@ struct LaneRoundIO {
   int32_t* tr_inds;
 };
 // `bins_in` == nullptr: level-0 edges torch.linspace(0, 1, S+1); else the scratch column written by the previous round.
-template <int LAYOUT = 0>
+// `e_tab`: the round's S+1 euclidean edges when they are the same for every ray (round 0 without per-ray nears / fars),
+// else nullptr.  TRACED = false: no trace pointer is set (the io.tr_* tests are not compiled in).
+template <int LAYOUT = 0, bool ACTORS = true, bool TRACED = true>
 NFF_D float lane_proposal_round(const RenderParams& P, const FieldGrids& fg, const LaneScratch& sc, int tid, int n_cand,
-                                const LaneRoundIO& io, const float* bins_in, const float o[3], const float d[3], float area,
-                                float s_near, float s_far, int64_t ray) {
+                                const LaneRoundIO& io, const float* bins_in, const float* e_tab, const float o[3],
+                                const float d[3], float area, float s_near, float s_far, int64_t ray) {
   const Sampling& sp = P.samp;
   const int S = io.S, S_new = io.S_new;
   auto edge = [bins_in, S](int i) { return bins_in ? bins_in[(size_t)i * kLaneThreads] : linspace01(i, S); };
+  auto euclid = [&](int i) { return e_tab ? e_tab[i] : to_euclid(edge(i), s_near, s_far, sp); };
   // running sums are kept in double: torch's CPU cumsum/cumprod (the oracle) accumulate in double
   // (acc_type<float, false>) and round per element; a sequential fp32 sum of 128 terms would be ~20x noisier
   double excl = 0.0, tot_d = 0.0;
   float depth_acc = 0.0f;
-  float e_prev = to_euclid(edge(0), s_near, s_far, sp);
+  float e_prev = euclid(0);
 #pragma unroll 1
   for (int s = 0; s < S; ++s) {
     const float T = expf(-(float)excl);
@@ -248,21 +252,21 @@ NFF_D float lane_proposal_round(const RenderParams& P, const FieldGrids& fg, con
     // weight of this round is exactly 0 whatever the density is (nan_to_num(x * 0) == 0) -- the gathers are skipped
     // when that holds for all 32 rays of the warp.  Not taken when per-sample actor ids are being traced.
     float w = 0.0f;
-    if (!(vote_all_converged(T == 0.0f) && io.tr_aid == nullptr)) {
+    if (!(vote_all_converged(T == 0.0f) && (!TRACED || io.tr_aid == nullptr))) {
       const float e0 = e_prev;
-      const float e1 = to_euclid(edge(s + 1), s_near, s_far, sp);
+      const float e1 = euclid(s + 1);
       e_prev = e1;
       Gauss g = sample_gaussian(o, d, area, e0, e1);
       int aid;
-      float dens = lane_proposal_density<LAYOUT>(fg, sc, tid, n_cand, g, &aid);
+      float dens = lane_proposal_density<LAYOUT, ACTORS>(fg, sc, tid, n_cand, g, &aid);
       float dd = fmul(fsub(e1, e0), dens);
       float alpha = fsub(1.0f, expf(-dd));
       excl += (double)dd;  // torch.cumsum order
       w = nan_to_num(fmul(alpha, T));
       depth_acc = fadd(depth_acc, fmul(w, fmul(fadd(e0, e1), 0.5f)));
-      if (io.tr_aid) io.tr_aid[ray * S + s] = aid;
+      if (TRACED && io.tr_aid) io.tr_aid[ray * S + s] = aid;
     }
-    if (io.tr_w) io.tr_w[ray * S + s] = w;
+    if (TRACED && io.tr_w) io.tr_w[ray * S + s] = w;
     w = fadd(w, sp.hist_pad);
     sc.w[(size_t)s * kLaneThreads + tid] = w;
     tot_d += (double)w;
@@ -295,9 +299,9 @@ NFF_D float lane_proposal_round(const RenderParams& P, const FieldGrids& fg, con
     t = fminf(fmaxf(t, 0.0f), 1.0f);
     const float nb = fadd(b0, fmul(t, fsub(b1, b0)));
     io.bins_out[(size_t)i * io.bins_stride] = nb;
-    if (io.tr_inds) io.tr_inds[ray * (S_new + 1) + i] = k;
-    if (io.tr_bins_s) io.tr_bins_s[ray * (S_new + 1) + i] = nb;
-    if (io.tr_bins_e) io.tr_bins_e[ray * (S_new + 1) + i] = to_euclid(nb, s_near, s_far, sp);
+    if (TRACED && io.tr_inds) io.tr_inds[ray * (S_new + 1) + i] = k;
+    if (TRACED && io.tr_bins_s) io.tr_bins_s[ray * (S_new + 1) + i] = nb;
+    if (TRACED && io.tr_bins_e) io.tr_bins_e[ray * (S_new + 1) + i] = to_euclid(nb, s_near, s_far, sp);
   }
   return depth_acc;
 }
@@ -508,6 +512,20 @@ struct LaneRay {
   float area, time, s_near, s_far;
   int n_cand;
 };
+// spacing-domain near / far of a ray (_get_ray_samples, neurad.py:443-449); rays without nears / fars use the defaults
+constexpr float kDefaultNear = 0.0f, kDefaultFar = 1.0e6f;
+NFF_D void lane_spacing_bounds(const Sampling& sp, float near_, float far_, float* s_near, float* s_far) {
+  *s_near = spacing_fn(near_, sp);
+  *s_far = spacing_fn(fminf(far_, sp.sky_distance), sp);
+}
+// Round 0's euclidean edge i (0 <= i <= kS0) of a bundle without nears / fars: the same for every ray, so the sampling kernel
+// computes the kS0+1 of them once per CTA instead of once per ray and sample.
+NFF_D float lane_round0_edge(const Sampling& sp, int i) {
+  float s_near, s_far;
+  lane_spacing_bounds(sp, kDefaultNear, kDefaultFar, &s_near, &s_far);
+  return to_euclid(linspace01(i, kS0), s_near, s_far, sp);
+}
+template <bool ACTORS = true>
 NFF_D LaneRay lane_ray_setup(const RenderParams& P, const LaneScratch& sc, int tid, int64_t ray) {
   const Sampling& sp = P.samp;
   LaneRay R;
@@ -519,13 +537,11 @@ NFF_D LaneRay lane_ray_setup(const RenderParams& P, const LaneScratch& sc, int t
   const bool lidar = P.rays.is_lidar ? P.rays.is_lidar[ray] != 0 : false;
   R.area = fmul(ldg(P.rays.pixel_area + ray), lidar ? 1.0f : sp.cam_area_scale);  // _scale_pixel_area (neurad.py:702-709)
   R.time = ldg(P.rays.times + ray);
-  float far_ = P.rays.fars ? ldg(P.rays.fars + ray) : 1.0e6f;  // _get_ray_samples (neurad.py:443-449)
-  far_ = fminf(far_, sp.sky_distance);
-  const float near_ = P.rays.nears ? ldg(P.rays.nears + ray) : 0.0f;
-  R.s_near = spacing_fn(near_, sp);
-  R.s_far = spacing_fn(far_, sp);
+  const float far_ = P.rays.fars ? ldg(P.rays.fars + ray) : kDefaultFar;
+  const float near_ = P.rays.nears ? ldg(P.rays.nears + ray) : kDefaultNear;
+  lane_spacing_bounds(sp, near_, far_, &R.s_near, &R.s_far);
   int overflow = 0;
-  R.n_cand = lane_actor_candidates(P.actors, R.time, R.o, R.d, sc, tid, &overflow);
+  R.n_cand = ACTORS ? lane_actor_candidates(P.actors, R.time, R.o, R.d, sc, tid, &overflow) : 0;
 #if defined(__CUDACC__)
   if (overflow && P.status) atomicExch(P.status, 3);
 #endif
@@ -534,30 +550,31 @@ NFF_D LaneRay lane_ray_setup(const RenderParams& P, const LaneScratch& sc, int t
 
 // Sampling stage: both proposal rounds (ProposalNetworkSampler.generate_ray_samples, ray_samplers.py:623-666).  The
 // final spacing edges go to this lane's column `bins2` (element i at bins2[i * bins2_stride]); prop depths to P.out.
-template <int LAYOUT = 0>
+// `e0_tab`: round 0's kS0+1 euclidean edges (lane_round0_edge) when the bundle has no per-ray nears / fars, else nullptr.
+template <int LAYOUT = 0, bool ACTORS = true, bool TRACED = true>
 NFF_D void sample_ray_lane(const RenderParams& P, const LaneScratch& sc, const LaneRay& R, int tid, int64_t ray, bool active,
-                           float* bins2, int64_t bins2_stride) {
+                           float* bins2, int64_t bins2_stride, const float* e0_tab = nullptr) {
   const Sampling& sp = P.samp;
-  float prop_depth[2];
 #pragma unroll 1
   for (int rd = 0; rd < 2; ++rd) {  // one copy of the round's code for both rounds (instruction-cache footprint)
-    LaneRoundIO io;
+    LaneRoundIO io{};
     io.S = rd == 0 ? kS0 : kS1;
     io.S_new = rd == 0 ? kS1 : kS2;
     io.u_tab = rd == 0 ? sp.u1 : sp.u2;
     io.bins_out = rd == 0 ? sc.bins1 + tid : bins2;
     io.bins_stride = rd == 0 ? (int64_t)kLaneThreads : bins2_stride;
-    io.tr_w = !active ? nullptr : rd == 0 ? P.trace.prop_weights_0 : P.trace.prop_weights_1;
-    io.tr_aid = !active ? nullptr : rd == 0 ? P.trace.actor_id_0 : P.trace.actor_id_1;
-    io.tr_bins_s = !active ? nullptr : rd == 0 ? P.trace.bins_s_1 : P.trace.bins_s_2;
-    io.tr_bins_e = !active ? nullptr : rd == 0 ? P.trace.bins_e_1 : P.trace.bins_e_2;
-    io.tr_inds = !active ? nullptr : rd == 0 ? P.trace.inds_1 : P.trace.inds_2;
-    prop_depth[rd] = lane_proposal_round<LAYOUT>(P, P.fields[sp.field_of_round[rd]], sc, tid, R.n_cand, io,
-                                         rd == 0 ? nullptr : sc.bins1 + tid, R.o, R.d, R.area, R.s_near, R.s_far, ray);
-  }
-  if (active) {
-    P.out.prop_depth_0[ray] = prop_depth[0];
-    P.out.prop_depth_1[ray] = prop_depth[1];
+    if (TRACED) {
+      io.tr_w = !active ? nullptr : rd == 0 ? P.trace.prop_weights_0 : P.trace.prop_weights_1;
+      io.tr_aid = !active ? nullptr : rd == 0 ? P.trace.actor_id_0 : P.trace.actor_id_1;
+      io.tr_bins_s = !active ? nullptr : rd == 0 ? P.trace.bins_s_1 : P.trace.bins_s_2;
+      io.tr_bins_e = !active ? nullptr : rd == 0 ? P.trace.bins_e_1 : P.trace.bins_e_2;
+      io.tr_inds = !active ? nullptr : rd == 0 ? P.trace.inds_1 : P.trace.inds_2;
+    }
+    const float prop_depth = lane_proposal_round<LAYOUT, ACTORS, TRACED>(
+        P, P.fields[sp.field_of_round[rd]], sc, tid, R.n_cand, io, rd == 0 ? nullptr : sc.bins1 + tid,
+        rd == 0 ? e0_tab : nullptr, R.o, R.d, R.area, R.s_near, R.s_far, ray);
+    // stored per round: a [2] array indexed by the rolled round counter would live in local memory
+    if (active) (rd == 0 ? P.out.prop_depth_0 : P.out.prop_depth_1)[ray] = prop_depth;
   }
 }
 
