@@ -127,6 +127,12 @@ int b200nerf_set_lidar_decoder(b200nerf_ctx* ctx, const float* w0, const float* 
 int b200nerf_set_appearance(b200nerf_ctx* ctx, const float* embedding, int num_embeds, int dim,
                             int embeds_per_sensor, float duration);
 
+/* The same embedding with use_temporal_appearance = False (neurad.py:190-195, 440): one row per sensor, and a ray's
+ * appearance columns are row `sensor_idx` copied.  Rays without sensor_idx use sensor 0 (the viewer's fallback sensor,
+ * neurad.py:425-428), as with b200nerf_set_appearance; sensor indices must be in [0, num_embeds), nothing checks them
+ * on the device.  Zero-copy; replaces a binding of b200nerf_set_appearance and vice versa. */
+int b200nerf_set_appearance_per_sensor(b200nerf_ctx* ctx, const float* embedding, int num_embeds, int dim);
+
 /* DynamicActors buffers/parameters (model_components/dynamic_actors.py:109-170): unique_timestamps [T],
  * actor_rotations_6d [T,A,6], actor_positions [T,A,3], actor_present_at_time [T,A] (uint8), actor_sizes
  * [A,3]; `padding_host` = actor_bbox_padding (3 floats, host).  n_actors == 0 disables the actor branch. */

@@ -48,9 +48,11 @@ def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
                                             actor_scale=float(src.actor.actor_scale), flip_prob=float(src.actor.flip_prob))
 
     sp = mc.sampling
-    if mc.num_proposal_rounds != 2 or not mc.field.use_sdf or not mc.use_temporal_appearance:
-        raise NotImplementedError("the b200 backend implements NeuRAD's default structure: 2 proposal rounds, SDF field, "
-                                  "temporal appearance embedding")
+    if mc.num_proposal_rounds != 2 or not mc.field.use_sdf:
+        raise NotImplementedError("the b200 backend implements NeuRAD's default structure: 2 proposal rounds, SDF field")
+    # `_num_embeds_per_sensor` exists only with temporal appearance (neurad.py:190-195)
+    n_emb = model.appearance_embedding.num_embeddings
+    num_sensors = n_emb // model._num_embeds_per_sensor if mc.use_temporal_appearance else n_emb
     return nsb.NeuRADConfig(
         grid=grid(mc.field.grid), proposal_grid_1=grid(sp.proposal_field_1.grid), proposal_grid_2=grid(sp.proposal_field_2.grid),
         sampling=nsb.SamplingSettings(num_proposal_samples=tuple(sp.num_proposal_samples), num_nerf_samples=sp.num_nerf_samples,
@@ -58,10 +60,10 @@ def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
                                       single_jitter=sp.single_jitter),
         geo_hidden_dim=mc.field.geo_hidden_dim, nff_hidden_dim=mc.field.nff_hidden_dim, nff_out_dim=mc.field.nff_out_dim,
         num_multisamples=mc.field.num_multisamples, appearance_dim=mc.appearance_dim,
+        use_temporal_appearance=bool(mc.use_temporal_appearance),
         temporal_appearance_freq=mc.temporal_appearance_freq, rgb_upsample_factor=mc.rgb_upsample_factor,
         rgb_hidden_dim=mc.rgb_hidden_dim, actor_bbox_padding=tuple(mc.dynamic_actors.actor_bbox_padding),
-        static_scale=float(model.scene_box.aabb.max()), duration=float(model._duration),
-        num_sensors=model.appearance_embedding.num_embeddings // model._num_embeds_per_sensor,
+        static_scale=float(model.scene_box.aabb.max()), duration=float(model._duration), num_sensors=num_sensors,
         n_actors=int(model.dynamic_actors.n_actors),
     )
 

@@ -187,9 +187,11 @@ class B200Backend:
             self._check(self.lib.b200nerf_set_lidar_decoder(self._h, *[_ptr(t) for t in ts]))
         emb = self._dev(p["appearance_embedding.weight"])
         self._keep["appearance"] = emb
-        self._check(
-            self.lib.b200nerf_set_appearance(self._h, _ptr(emb), emb.shape[0], emb.shape[1], cfg.embeds_per_sensor, float(cfg.duration))
-        )
+        if cfg.use_temporal_appearance:
+            self._check(self.lib.b200nerf_set_appearance(self._h, _ptr(emb), emb.shape[0], emb.shape[1], cfg.embeds_per_sensor,
+                                                         float(cfg.duration)))
+        else:
+            self._check(self.lib.b200nerf_set_appearance_per_sensor(self._h, _ptr(emb), emb.shape[0], emb.shape[1]))
         if n_act > 0:
             ts_ = self._dev(p["dynamic_actors.unique_timestamps"])
             rot = self._dev(p["dynamic_actors.actor_rotations_6d"])

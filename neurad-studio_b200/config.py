@@ -101,6 +101,9 @@ class NeuRADConfig:
     nff_out_dim: int = 32
     num_multisamples: int = 1  # NeuRADFieldConfig.num_multisamples, neurad_field.py:67
     appearance_dim: int = 16
+    # NeuRADModelConfig.use_temporal_appearance (neurad.py:136): True -> embeds_per_sensor rows per sensor, linearly
+    # interpolated in time; False (the paper presets) -> one row per sensor, copied
+    use_temporal_appearance: bool = True
     temporal_appearance_freq: float = 1.0
     rgb_upsample_factor: int = 3
     rgb_hidden_dim: int = 32
@@ -120,6 +123,11 @@ class NeuRADConfig:
     @property
     def embeds_per_sensor(self) -> int:
         return math.ceil(self.duration * self.temporal_appearance_freq)
+
+    @property
+    def num_appearance_embeds(self) -> int:
+        """Rows of appearance_embedding (neurad.py:190-195)."""
+        return self.num_sensors * self.embeds_per_sensor if self.use_temporal_appearance else self.num_sensors
 
     @property
     def feature_dim(self) -> int:
@@ -152,8 +160,37 @@ class ScaledCameraOptimizerConfig(CameraOptimizerConfig):
 
 
 def scaleopt_camera_optimizer() -> ScaledCameraOptimizerConfig:
-    """The camera optimizer of neurad-scaleopt / neurader-scaleopt / neuradest-scaleopt (method_configs.py:440-442)."""
-    return ScaledCameraOptimizerConfig(mode="SO3xR3", weights=(1.0, 1.0, 0.01, 0.01, 0.01, 1.0))
+    """The camera optimizer of neurad-scaleopt / neurader-scaleopt / neuradest-scaleopt (method_configs.py:440-449)."""
+    return ScaledCameraOptimizerConfig(mode="SO3xR3", weights=(1.0, 1.0, 0.01, 0.01, 0.01, 1.0), trans_l2_penalty=(1e-2, 1e-2, 1e-3))
+
+
+PRESETS = ("neurad", "neurad-scaleopt", "neurader", "neurader-scaleopt", "neuradest", "neuradest-scaleopt", "neurad-paper",
+           "neurad-2x-paper")
+
+
+def preset(name: str) -> Tuple[NeuRADConfig, CameraOptimizerConfig]:
+    """(model config, camera optimizer config) of one of the reference's NeuRAD method presets (method_configs.py:395-507).
+
+    - neurader / neuradest (+ -scaleopt) and neurad-2x-paper double every grid's static base / max resolution and add one
+      bit to every static and actor table (main static grid: levels 64 ... 16383, 2^23 rows).  neuradest only trains
+      longer than neurader, which is not part of this config.
+    - -scaleopt: the axis-weighted SO3xR3 camera optimizer.
+    - neurad-paper / neurad-2x-paper: one appearance embedding per sensor.  Their `f.flip_prob = 0.0` loop sets an
+      attribute the field configs do not read (the encoding reads `grid.actor.flip_prob`), so the actor flip probabilities
+      stay 0.25 / 0.5 in training, as in the reference."""
+    if name not in PRESETS:
+        raise ValueError(f"unknown preset {name!r}; known: {', '.join(PRESETS)}")
+    cfg = NeuRADConfig()
+    if name.startswith(("neurader", "neuradest")) or name == "neurad-2x-paper":
+        for g in (cfg.grid, *cfg.proposal_grids):
+            g.static.max_res *= 2
+            g.static.base_res *= 2
+            g.static.log2_hashmap_size += 1
+            g.actor.log2_hashmap_size += 1
+    if name.endswith("-paper"):
+        cfg.use_temporal_appearance = False
+    copt = scaleopt_camera_optimizer() if name.endswith("-scaleopt") else CameraOptimizerConfig(mode="off")
+    return cfg, copt
 
 
 def small_config(n_actors: int = 0, log2_main: int = 12, log2_prop: int = 11, **kw) -> NeuRADConfig:

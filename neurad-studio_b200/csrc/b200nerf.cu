@@ -99,6 +99,21 @@ int make_grid(const b200nerf_grid_desc* d, const float* table, Grid* g) {
   for (int i = 0; i < kMaxLevels; ++i) g->res[i] = i < d->num_levels ? d->scalings[i] : 0.f;
   return 0;
 }
+
+// The fused kernels address a level's rows by 32-bit byte offsets pre-multiplied into the hash (grid_cell_b /
+// cell_offsets_b: (h & mask) << log2(row bytes)), which is exact while log2 T + log2(4 F) <= 32.
+bool fused_table_fits(int log2_hashmap_size, int F) {
+  const int row_shift = F == 4 ? 4 : 2;
+  return log2_hashmap_size + row_shift <= 32;
+}
+
+// The tiny-cuda-nn kernels hold entry indices (level offset + index in the level, a dense level's before its wrap: below
+// twice its size) in 32 bits.
+bool tcnn_entries_fit(const b200nerf_tcnn_grid_desc* d) {
+  for (int l = 0; l < d->num_levels; ++l)
+    if ((uint64_t)d->offset[l] + 2ull * d->size[l] > (1ull << 32)) return false;
+  return true;
+}
 }  // namespace
 
 // =================================================================================================== kernels
@@ -1108,11 +1123,15 @@ int b200nerf_set_field_grids(b200nerf_ctx* c, int field, const b200nerf_grid_des
   if (fg.stat.L != wantL || fg.stat.F != wantF)
     return fail(B200NERF_ERR_UNSUPPORTED,
                 "fused kernel is specialised for NeuRAD's grid shapes (main: 8 levels x 4 features, proposal: 6 x 1)");
+  if (!fused_table_fits(sd->log2_hashmap_size, wantF))
+    return fail(B200NERF_ERR_UNSUPPORTED, "hash table too large for the fused kernels' 32-bit byte offsets");
   if (n_actors > 0) {
     REQUIRE(ad && atabs_host, "actor grid descriptor / tables missing");
     if (int e = make_grid(ad, nullptr, &fg.act)) return e;
     if (fg.act.L != 4 || fg.act.F != wantF)
       return fail(B200NERF_ERR_UNSUPPORTED, "actor grids must have 4 levels and the static grid's feature width");
+    if (!fused_table_fits(ad->log2_hashmap_size, wantF))
+      return fail(B200NERF_ERR_UNSUPPORTED, "actor hash table too large for the fused kernels' 32-bit byte offsets");
     cudaFree((void*)c->d_actor_tables[field]);
     c->d_actor_tables[field] = nullptr;
     CUDA_TRY(cudaMalloc((void**)&c->d_actor_tables[field], sizeof(float*) * n_actors));
@@ -1169,10 +1188,13 @@ int b200nerf_set_field_grids_tcnn(b200nerf_ctx* c, int field, const b200nerf_tcn
   if (fg.stat.L != wantL || fg.stat.F != wantF)
     return fail(B200NERF_ERR_UNSUPPORTED,
                 "fused kernel is specialised for NeuRAD's grid shapes (main: 8 levels x 4 features, proposal: 6 x 1)");
+  if (!tcnn_entries_fit(sd)) return fail(B200NERF_ERR_UNSUPPORTED, "tcnn grid has more entries than 32-bit indices address");
   if (n_actors > 0) {
     if (int e = make_tcnn_grid(ad, aparams, 4, &fg.act)) return e;
     if (fg.act.L != 4 || fg.act.F != wantF)
       return fail(B200NERF_ERR_UNSUPPORTED, "the 4-D actor grid must have 4 levels and the static grid's feature width");
+    if (!tcnn_entries_fit(ad))
+      return fail(B200NERF_ERR_UNSUPPORTED, "tcnn actor grid has more entries than 32-bit indices address");
   }
   fg.n_actors_f = (float)(n_actors > 0 ? n_actors : 1);
   fg.static_scale = static_scale;
@@ -1256,6 +1278,19 @@ int b200nerf_set_appearance(b200nerf_ctx* c, const float* emb, int num_embeds, i
   c->app.dim = dim;
   c->app.eps = eps;
   c->app.duration = duration;
+  c->have_app = true;
+  return 0;
+}
+
+int b200nerf_set_appearance_per_sensor(b200nerf_ctx* c, const float* emb, int num_embeds, int dim) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(dim >= 0 && dim <= kApp, "appearance_dim must be <= 16");
+  REQUIRE(dim == 0 || (emb && num_embeds > 0), "bad appearance embedding");
+  c->app.emb = emb;
+  c->app.num_embeds = num_embeds;
+  c->app.dim = dim;
+  c->app.eps = 0;          // the kernels' per-sensor branch
+  c->app.duration = 1.f;   // keeps the unused temporal index arithmetic finite
   c->have_app = true;
   return 0;
 }
@@ -2221,6 +2256,8 @@ int b200nerf_hashgrid_fwd(b200nerf_ctx* c, const b200nerf_grid_desc* desc, const
   DeviceGuard g(c->device);
   Grid gr{};
   if (int e = make_grid(desc, table, &gr)) return e;
+  if (indices && (uint64_t)gr.L * gr.T > (1ull << 31))
+    return fail(B200NERF_ERR_UNSUPPORTED, "row indices of more than 2^31 table rows do not fit int32");
   int64_t n = n_points * gr.L;
   hashgrid_fwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(gr, x, out, indices, n_points);
   CUDA_TRY(cudaGetLastError());

@@ -1094,9 +1094,10 @@ NFF_D void render_ray(const RenderParams& P, WS& ws, Mlp& mlp, int64_t ray, bool
   const int fdim = P.nff_dim + P.app.dim;
   float* fo = P.out.features + ray * fdim;
   fo[ln] = fsum;
-  // _get_appearance_embedding, temporal branch (neurad.py:423-441)
+  // _get_appearance_embedding (neurad.py:423-441); eps == 0: the per-sensor branch (:440), row `sensor_idx` copied
   float app = 0.0f;
   if (ln < P.app.dim) {
+    const bool per_sensor = P.app.eps == 0;
     float sens = P.rays.sensor_idx ? (float)P.rays.sensor_idx[ray] : 0.0f;
     float eps_ = (float)P.app.eps;
     float tidx = fmul(fdiv(time, P.app.duration), eps_);
@@ -1104,8 +1105,9 @@ NFF_D void render_ray(const RenderParams& P, WS& ws, Mlp& mlp, int64_t ray, bool
     float after = fminf(fmaxf(fadd(before, 1.0f), 0.0f), eps_ - 1.0f);
     float ratio = fsub(tidx, before);
     int ib = (int)fadd(before, fmul(sens, eps_)), ia = (int)fadd(after, fmul(sens, eps_));
+    if (per_sensor) ib = ia = (int)sens;
     float eb = ldg(P.app.emb + (size_t)ib * P.app.dim + ln), ea = ldg(P.app.emb + (size_t)ia * P.app.dim + ln);
-    app = fadd(fmul(eb, fsub(1.0f, ratio)), fmul(ea, ratio));
+    app = per_sensor ? eb : fadd(fmul(eb, fsub(1.0f, ratio)), fmul(ea, ratio));
     fo[P.nff_dim + ln] = app;
   }
   if (ln == 0) {

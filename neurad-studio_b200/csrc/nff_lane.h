@@ -664,7 +664,9 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
   float app[kApp];
 #pragma unroll
   for (int i = 0; i < kApp; ++i) app[i] = 0.0f;
-  if (P.app.dim > 0) {  // _get_appearance_embedding, temporal branch (neurad.py:423-441)
+  if (P.app.dim > 0) {  // _get_appearance_embedding (neurad.py:423-441)
+    // eps == 0: the per-sensor branch (:440), row `sensor_idx` copied; otherwise the temporal branch (:430-439)
+    const bool per_sensor = P.app.eps == 0;
     float sens = P.rays.sensor_idx ? (float)P.rays.sensor_idx[ray] : 0.0f;
     float eps_ = (float)P.app.eps;
     float tidx = fmul(fdiv(time, P.app.duration), eps_);
@@ -672,11 +674,12 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
     float after = fminf(fmaxf(fadd(before, 1.0f), 0.0f), eps_ - 1.0f);
     float ratio = fsub(tidx, before);
     int ib = (int)fadd(before, fmul(sens, eps_)), ia = (int)fadd(after, fmul(sens, eps_));
+    if (per_sensor) ib = ia = (int)sens;
 #pragma unroll
     for (int i = 0; i < kApp; ++i) {
       if (i < P.app.dim) {
         float eb = ldg(P.app.emb + (size_t)ib * P.app.dim + i), ea = ldg(P.app.emb + (size_t)ia * P.app.dim + i);
-        app[i] = fadd(fmul(eb, fsub(1.0f, ratio)), fmul(ea, ratio));
+        app[i] = per_sensor ? eb : fadd(fmul(eb, fsub(1.0f, ratio)), fmul(ea, ratio));
       }
     }
   }

@@ -98,6 +98,7 @@ struct Sampling {
 
 struct Appearance {
   const float* emb;
+  // eps: embeddings per sensor, interpolated in time; 0: one embedding per sensor, copied (use_temporal_appearance = False)
   int32_t num_embeds, dim, eps;
   float duration;
 };

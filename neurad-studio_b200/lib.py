@@ -89,6 +89,7 @@ SIGNATURES = {
     "b200nerf_set_main_mlps": (c_int, [c_void_p] + [c_void_p] * 10 + [c_float]),
     "b200nerf_set_lidar_decoder": (c_int, [c_void_p] + [c_void_p] * 6),
     "b200nerf_set_appearance": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float]),
+    "b200nerf_set_appearance_per_sensor": (c_int, [c_void_p, c_void_p, c_int, c_int]),
     "b200nerf_set_actors": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     POINTER(c_float)]),
     "b200nerf_set_sampling": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_float, c_float,

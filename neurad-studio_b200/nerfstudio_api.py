@@ -1295,12 +1295,21 @@ class NeuRADModel(nn.Module):
         return torch.bernoulli(torch.full((n_rays,), p, device=self.static_scale.device)) * -2 + 1
 
     def _get_appearance_embedding(self, ray_bundle: RayBundle, features: Tensor) -> Tensor:
-        """neurad.py:423-441: per-sensor embedding, linearly interpolated in time (temporal_appearance_freq)."""
+        """neurad.py:423-441: per-sensor embedding, linearly interpolated in time (temporal_appearance_freq), or with
+        use_temporal_appearance = False the sensor's one row."""
         sd = self.reference_state_dict()
         emb = sd["appearance_embedding.weight"]
         n = len(ray_bundle)
         sensor = ray_bundle.metadata.get("sensor_idxs")
         sensor = torch.zeros(n, dtype=torch.long, device=emb.device) if sensor is None else sensor.reshape(-1).long()
+        if not self.config.use_temporal_appearance:
+            if emb.requires_grad and emb.shape[0] <= 4096:
+                # training: a one-hot [N, E] @ [E, 16] product, for the same reason as below; the forward is exact (one
+                # nonzero term per row)
+                m = torch.zeros(n, emb.shape[0], device=emb.device, dtype=emb.dtype)
+                m.scatter_(1, sensor[:, None], 1.0)
+                return m @ emb
+            return emb[sensor]
         eps = self.config.embeds_per_sensor
         t = ray_bundle.times.reshape(-1) / self.config.duration * eps
         before = t.floor().clamp(0, eps - 1)

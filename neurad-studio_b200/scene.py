@@ -130,8 +130,7 @@ def make_params(
         grids(f"proposal_fields.{k}", g)
         w, _ = _linear(gen, 1, g.static.out_dim, bias=False, device=device)
         p[f"proposal_fields.{k}.density_decoder.weight"] = w
-    n_emb = cfg.num_sensors * cfg.embeds_per_sensor
-    p["appearance_embedding.weight"] = torch.randn(n_emb, cfg.appearance_dim, generator=gen, device=device)
+    p["appearance_embedding.weight"] = torch.randn(cfg.num_appearance_embeds, cfg.appearance_dim, generator=gen, device=device)
     for i, (o, n) in enumerate([(32, cfg.feature_dim), (32, 32), (2, 32)]):
         w, b = _linear(gen, o, n, device=device)
         p[f"lidar_decoder.layers.{i}.weight"], p[f"lidar_decoder.layers.{i}.bias"] = w, b
@@ -178,8 +177,7 @@ def make_params_tcnn(cfg: NeuRADConfig, seed: int = 0, table_scale: float = 1.0,
         grids(f"proposal_fields.{k}", g)
         w, _ = _linear(gen, 1, g.static.out_dim, bias=False, device=device)
         p[f"proposal_fields.{k}.density_decoder.weight"] = w
-    n_emb = cfg.num_sensors * cfg.embeds_per_sensor
-    p["appearance_embedding.weight"] = torch.randn(n_emb, cfg.appearance_dim, generator=gen, device=device)
+    p["appearance_embedding.weight"] = torch.randn(cfg.num_appearance_embeds, cfg.appearance_dim, generator=gen, device=device)
     mlp("lidar_decoder", cfg.feature_dim, 32, 3, 2)
     if cfg.n_actors > 0:
         trajs = trajectories if trajectories is not None else make_trajectories(cfg.n_actors, cfg.duration, seed=seed)

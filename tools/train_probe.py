@@ -67,12 +67,20 @@ def main():
     ap.add_argument("--small-tables", action="store_true", help="2^14 / 2^13 slot tables instead of NeuRAD's 2^22 / 2^20")
     ap.add_argument("--camopt", choices=("off", "so3xr3", "scaled"), default="off")
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--preset", choices=nsb.PRESETS, default=None,
+                    help="the model config and camera optimizer of a reference preset (overrides --camopt and the table sizes)")
     a = ap.parse_args()
     dev = "cuda"
     cfg = nsb.small_config(n_actors=a.actors, log2_main=14, log2_prop=13) if a.small_tables else nsb.NeuRADConfig(n_actors=a.actors)
+    preset_copt = None
+    if a.preset is not None:
+        cfg, preset_copt = nsb.preset(a.preset)
+        cfg.n_actors = a.actors
     trajs = scene.make_trajectories(a.actors, cfg.duration) if a.actors else None
     params = scene.make_params(cfg, seed=1, beta=3.0, sdf_bias=0.6, trajectories=trajs)
     copt = {"off": None, "so3xr3": CameraOptimizerConfig(mode="SO3xR3"), "scaled": scaleopt_camera_optimizer()}[a.camopt]
+    if preset_copt is not None:
+        copt = None if preset_copt.mode == "off" else preset_copt
     model = NeuRADModel(cfg, trajs, camera_optimizer=copt, num_cameras=cfg.num_sensors)
     params.update({"camera_optimizer." + k: v for k, v in model.camera_optimizer.state_dict().items()})
     model.load_reference_state_dict(params)
@@ -116,7 +124,7 @@ def main():
     med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
     total = med["forward_and_losses"] + med["backward"]
     res = {"what": "NFF training step (module walk + hand-written backward operators), device time", "rays": n,
-           "cam_rays": a.cam_rays, "lidar_rays": a.lidar_rays, "actors": a.actors, "tables": "small" if a.small_tables else "neurad-default",
+           "cam_rays": a.cam_rays, "lidar_rays": a.lidar_rays, "actors": a.actors, "tables": a.preset or ("small" if a.small_tables else "neurad-default"),
            "ms": med, "ms_total": total, "rays_per_s": n / total * 1e3, "loss": float(loss.detach()), "camopt": a.camopt,
            "gpu": torch.cuda.get_device_name(), "kernels": kernels}
     print(json.dumps(res))
