@@ -573,6 +573,19 @@ int b200nerf_raygen_lidar_grid(b200nerf_ctx* ctx, const float* l2w_host, float e
                                float revolution_time, const float* velocity_host, float h_div, float v_div,
                                float* origins, float* directions, float* pixel_area, float* times, void* stream);
 
+/* ---- lidar evaluation ----------------------------------------------------------------------------------- */
+
+/* Chamfer distance of NeuRAD's lidar metrics (utils/math.py:745-798, models/neurad.py:614-618): src [n_src, src_stride]
+ * and dst [n_dst, dst_stride] hold (x, y, z, ...) rows in fp32.  min_src[i] = min_j |src_i - dst_j|^2 and
+ * min_dst[j] = min_i |dst_j - src_i|^2, exact fp32 from direct differences (no |a|^2 + |b|^2 - 2ab); a NaN coordinate
+ * gives NaN for its point and every point whose candidate set contains it.  Both arrays are required: they are also the
+ * working storage of the reduction.  *out_scalar (device, fp64) = sum(min_src) + sum(min_dst), each sum taken in fp64 in
+ * a fixed order (bit-reproducible); with normalize_by_dst both sums are divided by n_dst, the reference's normalisation.
+ * Empty clouds and more than 2^31 - 1 points are rejected (B200NERF_ERR_INVALID). */
+int b200nerf_chamfer_distance(b200nerf_ctx* ctx, const float* src, int64_t n_src, int src_stride, const float* dst,
+                              int64_t n_dst, int dst_stride, int normalize_by_dst, double* out_scalar, float* min_src,
+                              float* min_dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -64,7 +64,7 @@ def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
         temporal_appearance_freq=mc.temporal_appearance_freq, rgb_upsample_factor=mc.rgb_upsample_factor,
         rgb_hidden_dim=mc.rgb_hidden_dim, actor_bbox_padding=tuple(mc.dynamic_actors.actor_bbox_padding),
         static_scale=float(model.scene_box.aabb.max()), duration=float(model._duration), num_sensors=num_sensors,
-        n_actors=int(model.dynamic_actors.n_actors),
+        n_actors=int(model.dynamic_actors.n_actors), ray_drop_loss_mult=float(mc.loss.ray_drop_loss_mult),
     )
 
 
@@ -92,6 +92,9 @@ class B200NeuRADModel(NeuRADModel):
         super().populate_modules()
         self._b200_uid = next(_api._UIDS)
         self._b200_cfg: Optional[nsb.NeuRADConfig] = None
+        # the lidar metrics of the inherited get_image_metrics_and_images (neurad.py:271, 616-618): the library's exact
+        # all-pairs kernel instead of chunked torch.cdist, same arguments and value
+        self.chamfer_distance = lambda pred, gt: nsb.chamfer_distance(pred, gt, 1_000, True)
 
     # ---------------------------------------------------------------------------------------------- binding
     _B200_PREFIXES = ("field.", "proposal_fields.", "lidar_decoder.", "appearance_embedding.", "dynamic_actors.")

@@ -934,3 +934,27 @@ class B200Backend:
                                                 3.0e-3, 1.5e-3, _ptr(o), _ptr(d), _ptr(a), _ptr(t), self._stream)
         )
         return {"origins": o, "directions": d, "pixel_area": a, "times": t, "shape": (beams, n_az)}
+
+    # ------------------------------------------------------------------------------------------ lidar evaluation
+    def chamfer_distance(self, pred: torch.Tensor, gt: torch.Tensor, normalize_with_target: bool = True,
+                         want_minima: bool = False):
+        """Chamfer distance between point clouds pred [N,>=3] and gt [M,>=3] (x, y, z in the first three columns; a row
+        stride is fine, so `points[..., :3]` of an [N,4] tensor needs no copy): sum_i min_j |p_i - g_j|^2 +
+        sum_j min_i |g_j - p_i|^2, both sums divided by M with `normalize_with_target` (utils/math.py:783-796).
+        Exact fp32 per-pair values, fp64 sums in a fixed order; returns a 0-d float64 tensor on the device, and with
+        `want_minima` also the per-point minima [N] and [M] (fp32).  Empty clouds raise B200NerfError."""
+        def rows(t):
+            t = t.detach()
+            if t.device != self.device or t.dtype != torch.float32 or t.dim() != 2 or t.shape[1] < 3 or t.stride(1) != 1:
+                t = self._dev(t.reshape(-1, t.shape[-1]))
+            return t
+
+        p, g = rows(pred), rows(gt)
+        n, m = p.shape[0], g.shape[0]
+        out = torch.empty((), dtype=torch.float64, device=self.device)
+        min_p = torch.empty(max(n, 1), device=self.device)[:n]
+        min_g = torch.empty(max(m, 1), device=self.device)[:m]
+        self._check(self.lib.b200nerf_chamfer_distance(self._h, _ptr(p), n, p.stride(0), _ptr(g), m, g.stride(0),
+                                                       int(bool(normalize_with_target)), _ptr(out), _ptr(min_p), _ptr(min_g),
+                                                       self._stream))
+        return (out, min_p, min_g) if want_minima else out

@@ -110,6 +110,9 @@ class NeuRADConfig:
     actor_bbox_padding: Tuple[float, float, float] = (0.25, 0.25, 0.1)
     carving_epsilon: float = 0.1  # LossSettings (neurad.py:79,87): lidar carving masks of the training outputs
     non_return_lidar_distance: float = 150.0
+    # LossSettings.ray_drop_loss_mult (neurad.py:91); the lidar metrics' predicted returns are ray-drop probabilities < 0.5
+    # when it is > 0, depths < non_return_lidar_distance otherwise (neurad.py:610-613)
+    ray_drop_loss_mult: float = 0.01
     # scene-level constants (dataset metadata in the reference)
     static_scale: float = 100.0
     duration: float = 8.0

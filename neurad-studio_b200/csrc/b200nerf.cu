@@ -12,6 +12,7 @@
 #include "nff_lane.h"
 #include "rgb_decoder.cuh"
 #include "modules.cuh"
+#include "lidar_eval.cuh"
 
 using namespace nff;
 
@@ -2403,6 +2404,47 @@ int b200nerf_raygen_lidar_grid(b200nerf_ctx* c, const float* l2w_host, float ele
   if (velocity_host) memcpy(a.vel, velocity_host, sizeof(float) * 3);
   int64_t n = (int64_t)beams * n_azimuth;
   raygen_lidar_grid_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, origins, directions, pixel_area, times);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---- lidar evaluation (lidar_eval.cuh)
+// Target splits of one direction: about 8 CTAs per SM in all, never more splits than target tiles.
+static int chamfer_tiles_per_split(int sm_count, int64_t n_src, int64_t n_dst) {
+  const int64_t blocks_x = (n_src + kChamferThreads * kChamferPts - 1) / (kChamferThreads * kChamferPts);
+  const int64_t n_tiles = (n_dst + kChamferTile - 1) / kChamferTile;
+  int64_t splits = (8 * (int64_t)sm_count + blocks_x - 1) / blocks_x;
+  splits = splits < 1 ? 1 : splits > n_tiles ? n_tiles : splits;
+  return (int)((n_tiles + splits - 1) / splits);
+}
+
+static void chamfer_direction(const b200nerf_ctx* c, const float* src, int64_t n_src, int src_stride, const float* dst,
+                              int64_t n_dst, int dst_stride, float* min_out, cudaStream_t s) {
+  const int tps = chamfer_tiles_per_split(c->sm_count, n_src, n_dst);
+  const int64_t n_tiles = (n_dst + kChamferTile - 1) / kChamferTile;
+  const dim3 grid((unsigned)((n_src + kChamferThreads * kChamferPts - 1) / (kChamferThreads * kChamferPts)),
+                  (unsigned)((n_tiles + tps - 1) / tps));
+  chamfer_min_kernel<<<grid, kChamferThreads, 0, s>>>(src, (int)n_src, src_stride, dst, (int)n_dst, dst_stride, tps,
+                                                     reinterpret_cast<unsigned*>(min_out));
+}
+
+int b200nerf_chamfer_distance(b200nerf_ctx* c, const float* src, int64_t n_src, int src_stride, const float* dst,
+                              int64_t n_dst, int dst_stride, int normalize_by_dst, double* out_scalar, float* min_src,
+                              float* min_dst, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n_src >= 1 && n_dst >= 1, "chamfer distance of an empty point cloud");
+  REQUIRE(n_src <= 0x7fffffff && n_dst <= 0x7fffffff, "point clouds of more than 2^31 - 1 points are not supported");
+  REQUIRE(src_stride >= 3 && dst_stride >= 3, "points need at least x,y,z");
+  REQUIRE(src && dst && out_scalar && min_src && min_dst, "NULL argument");
+  DeviceGuard g(c->device);
+  const cudaStream_t s = (cudaStream_t)stream;
+  CUDA_TRY(cudaMemsetAsync(min_src, 0xff, sizeof(float) * n_src, s));
+  CUDA_TRY(cudaMemsetAsync(min_dst, 0xff, sizeof(float) * n_dst, s));
+  chamfer_direction(c, src, n_src, src_stride, dst, n_dst, dst_stride, min_src, s);
+  chamfer_direction(c, dst, n_dst, dst_stride, src, n_src, src_stride, min_dst, s);
+  chamfer_reduce_kernel<<<1, kChamferReduceThreads, 0, s>>>(reinterpret_cast<unsigned*>(min_src), (int)n_src,
+                                                            reinterpret_cast<unsigned*>(min_dst), (int)n_dst,
+                                                            normalize_by_dst, out_scalar);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

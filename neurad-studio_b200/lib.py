@@ -169,6 +169,8 @@ SIGNATURES = {
     "b200nerf_raygen_lidar_points": (c_int, [c_void_p, POINTER(c_float), c_void_p, c_int, c_int64, c_float,
                                              POINTER(c_float), c_float, c_float, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_void_p, c_void_p]),
+    "b200nerf_chamfer_distance": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int64, c_int, c_int, c_void_p,
+                                          c_void_p, c_void_p, c_void_p]),
 }
 
 _LIB = None

@@ -39,6 +39,7 @@ import torch
 from torch import Tensor, nn
 
 from . import autograd as AG
+from . import metrics as M
 from .backend import B200Backend
 from .config import CameraOptimizerConfig, HashGridSettings, NeuRADConfig, ScaledCameraOptimizerConfig
 
@@ -1067,6 +1068,9 @@ class NeuRADModel(nn.Module):
         # ad_model.py:70-72; state dict keys camera_optimizer.pose_adjustment (+ .weights) as in the reference
         self.camera_optimizer = make_camera_optimizer(camera_optimizer, num_cameras, non_trainable_camera_indices=non_trainable_camera_indices)
         self.use_camopt_in_eval = use_camopt_in_eval
+        # lidar metrics (neurad.py:268-271); the chamfer distance runs on the library's all-pairs kernel
+        self.median_l2, self.mean_rel_l2, self.rmse = M.median_l2, M.mean_rel_l2, M.rmse
+        self.chamfer_distance = lambda pred, gt: M.chamfer_distance(pred, gt, 1_000, True)
 
     # -- nn.Module state dict in the reference's key format --------------------------------------------------------
     @staticmethod
@@ -1403,6 +1407,48 @@ class NeuRADModel(nn.Module):
         pts = ray_bundle.origins + ray_bundle.directions * outputs["depth"]
         outputs["points"] = pts @ rot_t.t() - (rot_t @ l2w[:3, 3])
         return outputs, batch
+
+    @torch.no_grad()
+    def get_image_metrics_and_images(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor]) -> Tuple[Dict[str, float], Dict[str, Tensor]]:
+        """The lidar half of neurad.py:563-621, on the outputs / batch of get_outputs_for_lidar: depth median L2, depth mean
+        relative L2, intensity RMSE, ray-drop accuracy and chamfer distance, with the reference's keys and values.  Like the
+        reference it fills batch["is_lidar"] / batch["did_return"] when they are absent, and the chamfer distance is a 0-d
+        tensor (the mean range of the measured returns) when there are no predicted or no measured returns, a float
+        otherwise.  images_dict stays empty.
+
+        A camera batch ("image") raises: PSNR / SSIM / LPIPS need torchmetrics and LPIPS weights, which this library does
+        not ship, and partial camera metrics are never returned."""
+        if "image" in batch:
+            raise NotImplementedError("camera metrics (PSNR / SSIM / LPIPS) need torchmetrics and LPIPS weights, which "
+                                      "neurad_studio_b200 does not ship; evaluate camera images with the reference's model")
+        metrics_dict: Dict[str, float] = {}
+        images_dict: Dict[str, Tensor] = {}
+        if "lidar" in batch:
+            device = self.static_scale.device
+            points = batch["lidar"].to(device)
+            if "is_lidar" not in batch:
+                batch["is_lidar"] = torch.ones(*batch["lidar"].shape[:-1], 1, dtype=torch.bool, device=device)
+            if "did_return" not in batch:
+                batch["did_return"] = torch.ones(*batch["lidar"].shape[:-1], 1, dtype=torch.bool, device=device)
+            ray_drop_logits = outputs["ray_drop_logits"]
+            pred_depth = outputs["depth"]
+            did_return = batch["did_return"][:, 0].to(device)
+            is_lidar = batch["is_lidar"][:, 0].to(device)
+            # the reference's indexing: [is_lidar] then [did_return], which needs every ray of the batch to be a lidar ray
+            metrics_dict["depth_median_l2"] = float(self.median_l2(pred_depth[is_lidar][did_return], batch["distance"][did_return]))
+            metrics_dict["depth_mean_rel_l2"] = float(self.mean_rel_l2(pred_depth[is_lidar][did_return], batch["distance"][did_return]))
+            metrics_dict["intensity_rmse"] = float(self.rmse(outputs["intensity"][did_return], points[did_return, 3:4]))
+            metrics_dict["ray_drop_accuracy"] = float(((ray_drop_logits.sigmoid() > 0.5).squeeze(-1) == ~did_return).float().mean())
+            if self.config.ray_drop_loss_mult > 0.0:
+                pred_points_did_return = (ray_drop_logits.sigmoid() < 0.5).squeeze(-1)
+            else:
+                pred_points_did_return = (pred_depth < self.config.non_return_lidar_distance).squeeze(-1)
+            if pred_points_did_return.any() and points.shape[0] > 0 and did_return.any():
+                pred_points = outputs["points"][is_lidar][pred_points_did_return]
+                metrics_dict["chamfer_distance"] = float(self.chamfer_distance(pred_points[..., :3], points[did_return, :3]))
+            else:
+                metrics_dict["chamfer_distance"] = points[did_return, :3].norm(dim=-1).mean()
+        return metrics_dict, images_dict
 
     @torch.no_grad()
     def get_outputs_for_camera_ray_bundle(self, camera_ray_bundle: RayBundle) -> Dict[str, Tensor]:
