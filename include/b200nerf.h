@@ -543,6 +543,23 @@ int64_t b200nerf_rgb_decode_workspace_bytes(int batch, int height, int width);
 int b200nerf_rgb_decode_fwd(b200nerf_ctx* ctx, const float* features, int batch, int height, int width, float* rgb,
                             void* workspace, int64_t workspace_bytes, int impl, void* stream);
 
+/* One of the ten launches of b200nerf_rgb_decode_fwd (which is exactly these ten calls), for testing a layer on its own.
+ * Activations between layers use the "ACT" layout: 128 B per pixel, [batch][height][width][8 chunks][8 bf16]; chunk c < 4
+ * holds bf16(v) (the "hi" part, round to nearest even) of channels 8c..8c+7, chunk 4 + c holds bf16(v - hi) (the "lo"
+ * part) of the same channels, so hi + lo carries 16 significant bits of v.  `height` and `width` are the layer's INPUT
+ * resolution.  Layers:
+ *   0      rgb_decoder.0/.1: 1x1 conv + ReLU, in = fp32 features [batch,height,width,in_dim] -> out = ACT
+ *   1, 2   rgb_decoder.2 (the two 7x7 convs of the BasicBlock), ACT -> ACT
+ *   3, 4   rgb_decoder.3
+ *   5      rgb_decoder.4: ConvTranspose2d, ACT [batch,height,width] -> ACT [batch,3*height,3*width]
+ *   6, 7   rgb_decoder.5
+ *   8, 9   rgb_decoder.6; layer 9 also runs rgb_decoder.7/.8 (1x1 conv + sigmoid): out = fp32 rgb [batch,height,width,3]
+ * `residual` (the BasicBlock input, ACT at the layer's resolution) is required for layers 2, 4, 7 and 9 and must be NULL
+ * for the others.  ACT buffers must be 16-byte aligned; `in` may not be `out`.  impl as for b200nerf_rgb_decode_fwd; it
+ * selects the kernel of the 7x7 layers only (layers 0 and 5 have one implementation). */
+int b200nerf_rgb_decode_layer(b200nerf_ctx* ctx, int layer, const void* in, const void* residual, void* out, int batch, int height,
+                              int width, int impl, void* stream);
+
 /* ---- ray generation ------------------------------------------------------------------------------------- */
 
 /* Cameras.generate_rays for one PERSPECTIVE camera without distortion, top-to-bottom rolling shutter

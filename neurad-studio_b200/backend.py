@@ -864,6 +864,34 @@ class B200Backend:
                                                      {"tc": 0, "ref": 1, "tc_ldgsts": 2}[impl], self._stream))
         return rgb
 
+    def rgb_decode_layer(self, layer: int, x: torch.Tensor, residual: Optional[torch.Tensor] = None, impl: str = "tc",
+                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """One of rgb_decode's ten launches (b200nerf_rgb_decode_layer).  Activations are ACT tensors: bf16 [B,H,W,64],
+        elements 0..31 the hi parts (bf16 of the value) of the 32 channels, 32..63 their lo parts (bf16 of value - hi),
+        which is the library's 128-byte ACT pixel.  Layer 0 takes fp32 features [B,H,W,in_dim]; layer 5 returns
+        [B,3H,3W,64]; layer 9 returns fp32 rgb [B,H,W,3].  `residual` (ACT) is required for layers 2, 4, 7 and 9."""
+        if not 0 <= layer <= 9:
+            raise _lib.B200NerfError("layer must be in [0, 9]")
+        want = torch.float32 if layer == 0 else torch.bfloat16
+        if x.dtype != want or x.device != self.device or not x.is_contiguous() or x.dim() != 4:
+            raise _lib.B200NerfError(f"rgb_decode_layer: input must be a contiguous {want} [B,H,W,C] tensor on the backend's device")
+        b, h, w, c = x.shape
+        if c != (getattr(self, "_dec_in_dim", None) if layer == 0 else 64):
+            raise _lib.B200NerfError(f"rgb_decode_layer: layer {layer} input has {c} channels")
+        if residual is not None and (residual.dtype != torch.bfloat16 or residual.shape != x.shape or not residual.is_contiguous()
+                                     or residual.device != self.device):
+            raise _lib.B200NerfError("rgb_decode_layer: residual must be an ACT tensor shaped like the input")
+        up = 3 if layer == 5 else 1
+        shape = (b, h * up, w * up, 3 if layer == 9 else 64)
+        dtype = torch.float32 if layer == 9 else torch.bfloat16
+        if out is None:
+            out = torch.empty(shape, dtype=dtype, device=self.device)
+        if out.shape != shape or out.dtype != dtype or not out.is_contiguous() or out.device != self.device:
+            raise _lib.B200NerfError(f"rgb_decode_layer: `out` must be a contiguous {dtype} {list(shape)} tensor")
+        self._check(self.lib.b200nerf_rgb_decode_layer(self._h, layer, _ptr(x), _ptr(residual), _ptr(out), b, h, w,
+                                                       {"tc": 0, "ref": 1, "tc_ldgsts": 2}[impl], self._stream))
+        return out
+
     # ------------------------------------------------------------------------------------------- ray generation
     def _ray_buffers(self, n: int, out: Optional[Dict[str, torch.Tensor]]):
         if out is None:

@@ -2131,6 +2131,76 @@ int64_t b200nerf_rgb_decode_workspace_bytes(int batch, int height, int width) {
   return 3 * act_bytes(lo) + 3 * act_bytes(lo * dec::kUp * dec::kUp);
 }
 
+int b200nerf_rgb_decode_layer(b200nerf_ctx* c, int layer, const void* in, const void* residual, void* out, int batch, int height,
+                              int width, int impl, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(layer >= 0 && layer <= 9, "layer must be in [0, 9]");
+  REQUIRE(batch >= 0 && height >= 0 && width >= 0, "negative image shape");
+  REQUIRE(impl >= 0 && impl <= 2, "impl: 0 = wgmma + TMA loads, 1 = CUDA-core fp32 cross-check, 2 = wgmma + LDGSTS loads");
+  if (!c->have_rgb_decoder) return fail(B200NERF_ERR_STATE, "set_rgb_decoder was not called");
+  const bool has_res = layer == 2 || layer == 4 || layer == 7 || layer == 9;
+  REQUIRE(has_res == (residual != nullptr), "a residual is required for layers 2, 4, 7 and 9 and rejected for the others");
+  if (batch == 0 || height == 0 || width == 0) return 0;
+  REQUIRE(in && out, "NULL argument");
+  REQUIRE(in != out, "the layer cannot run in place");
+  // ACT buffers are read by the TMA engine (16-byte aligned global address); features and rgb are plain fp32 arrays
+  REQUIRE(((uintptr_t)in & (layer == 0 ? 3 : 15)) == 0, "input must be 16-byte aligned (4-byte for layer 0's features)");
+  REQUIRE(((uintptr_t)residual & 15) == 0, "residual must be 16-byte aligned");
+  REQUIRE(((uintptr_t)out & (layer == 9 ? 3 : 15)) == 0, "output must be 16-byte aligned (4-byte for layer 9's rgb)");
+  DeviceGuard g(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t px = (int64_t)batch * height * width;
+  const DecSmall d = dec_small(c->d_dec_small);
+  if (layer == 0) {  // rgb_decoder.0/.1
+    dec::dec_input_kernel<<<(unsigned)((px + 127) / 128), 128, sizeof(float) * (c->dec_in_dim * dec::kC + dec::kC), st>>>(
+        (const float*)in, px, c->dec_in_dim, d.in_w, d.in_b, (uint4*)out);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  }
+  if (layer == 5) {  // rgb_decoder.4: 3x transposed conv
+    dec::dec_upsample_kernel<<<(unsigned)((px + 2 * dec::kUpThreads - 1) / (2 * dec::kUpThreads)), dec::kUpThreads,
+                               sizeof(float) * (9 * dec::kC * dec::kC + dec::kC), st>>>((const uint4*)in, batch, height, width, d.up_w,
+                                                                                       d.up_b, (uint4*)out);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  }
+  // the 7x7 convs of rgb_decoder.2, .3 (layers 1-4) and .5, .6 (layers 6-9; .7/.8 fused into layer 9's epilogue)
+  const int conv = layer < 5 ? layer - 1 : layer - 2, H = height, W = width;
+  const int epi = layer == 9 ? dec::EPI_RES_RELU_RGB : has_res ? dec::EPI_RES_RELU : dec::EPI_RELU;
+  dec::ConvArgs a{};
+  a.in = (const uint4*)in; a.residual = (const uint4*)residual;
+  a.out_act = layer == 9 ? nullptr : (uint4*)out; a.out_rgb = layer == 9 ? (float*)out : nullptr;
+  a.w_img = c->d_dec_wimg[conv]; a.w_f32 = c->d_dec_wf32[conv]; a.bias = c->d_dec_bias + conv * dec::kC;
+  a.out_w = d.out_w; a.out_b = d.out_b;
+  a.batch = batch; a.H = H; a.W = W; a.status = c->d_status;
+  if (impl == 0) {
+    dec::ConvArgsTma t{};
+    t.a = a;
+    if (!act_window_map(&t.in_map, in, batch, H, W)) return fail(B200NERF_ERR_CUDA, "cuTensorMapEncodeTiled failed for the decoder's input window");
+    const int64_t tiles = (int64_t)batch * ((H + dec::kTH - 1) / dec::kTH) * ((W + dec::kStrip - 1) / dec::kStrip);
+    const int grid = (int)(tiles < c->sm_count ? tiles : c->sm_count);
+    const size_t smem = sizeof(dec::ConvSmem);
+    if (epi == dec::EPI_RELU) dec::dec_conv7_tma_kernel<dec::EPI_RELU><<<grid, dec::kConvThreads, smem, st>>>(t);
+    else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_tma_kernel<dec::EPI_RES_RELU><<<grid, dec::kConvThreads, smem, st>>>(t);
+    else dec::dec_conv7_tma_kernel<dec::EPI_RES_RELU_RGB><<<grid, dec::kConvThreads, smem, st>>>(t);
+  } else if (impl == 2) {
+    const int64_t tiles = (int64_t)batch * ((H + dec::kTH - 1) / dec::kTH) * ((W + dec::kStrip - 1) / dec::kStrip);
+    const int grid = (int)(tiles < c->sm_count ? tiles : c->sm_count);
+    const size_t smem = sizeof(dec::ConvSmem);
+    if (epi == dec::EPI_RELU) dec::dec_conv7_tc_kernel<dec::EPI_RELU><<<grid, dec::kConvThreads, smem, st>>>(a);
+    else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_tc_kernel<dec::EPI_RES_RELU><<<grid, dec::kConvThreads, smem, st>>>(a);
+    else dec::dec_conv7_tc_kernel<dec::EPI_RES_RELU_RGB><<<grid, dec::kConvThreads, smem, st>>>(a);
+  } else {
+    const unsigned grid = (unsigned)((int64_t)batch * H * ((W + 127) / 128));
+    if (epi == dec::EPI_RELU) dec::dec_conv7_ref_kernel<dec::EPI_RELU><<<grid, 128, 0, st>>>(a);
+    else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_ref_kernel<dec::EPI_RES_RELU><<<grid, 128, 0, st>>>(a);
+    else dec::dec_conv7_ref_kernel<dec::EPI_RES_RELU_RGB><<<grid, 128, 0, st>>>(a);
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B200NERF_ERR_CUDA, cudaGetErrorString(e));
+  return 0;
+}
+
 int b200nerf_rgb_decode_fwd(b200nerf_ctx* c, const float* features, int batch, int height, int width, float* rgb,
                             void* workspace, int64_t workspace_bytes, int impl, void* stream) {
   REQUIRE(c, "ctx is NULL");
@@ -2141,67 +2211,31 @@ int b200nerf_rgb_decode_fwd(b200nerf_ctx* c, const float* features, int batch, i
   REQUIRE(features && rgb && workspace, "NULL argument");
   REQUIRE(workspace_bytes >= b200nerf_rgb_decode_workspace_bytes(batch, height, width), "workspace too small (see b200nerf_rgb_decode_workspace_bytes)");
   REQUIRE(((uintptr_t)workspace & 15) == 0, "workspace must be 16-byte aligned");
-  DeviceGuard g(c->device);
-  cudaStream_t st = (cudaStream_t)stream;
   const int64_t lo_px = (int64_t)batch * height * width, hi_px = lo_px * dec::kUp * dec::kUp;
   unsigned char* ws = (unsigned char*)workspace;
   uint4* lo[3];
   uint4* hi[3];
   for (int i = 0; i < 3; ++i) lo[i] = (uint4*)(ws + i * act_bytes(lo_px));
   for (int i = 0; i < 3; ++i) hi[i] = (uint4*)(ws + 3 * act_bytes(lo_px) + i * act_bytes(hi_px));
-  const DecSmall d = dec_small(c->d_dec_small);
-  dec::dec_input_kernel<<<(unsigned)((lo_px + 127) / 128), 128, sizeof(float) * (c->dec_in_dim * dec::kC + dec::kC), st>>>(
-      features, lo_px, c->dec_in_dim, d.in_w, d.in_b, lo[0]);
-  CUDA_TRY(cudaGetLastError());
-  auto conv = [&](int layer, int epi, const uint4* in, const uint4* res, uint4* out, float* out_rgb, int H, int W) -> int {
-    dec::ConvArgs a{};
-    a.in = in; a.residual = res; a.out_act = out; a.out_rgb = out_rgb;
-    a.w_img = c->d_dec_wimg[layer]; a.w_f32 = c->d_dec_wf32[layer]; a.bias = c->d_dec_bias + layer * dec::kC;
-    a.out_w = d.out_w; a.out_b = d.out_b;
-    a.batch = batch; a.H = H; a.W = W; a.status = c->d_status;
-    if (impl == 0) {
-      dec::ConvArgsTma t{};
-      t.a = a;
-      if (!act_window_map(&t.in_map, in, batch, H, W)) return fail(B200NERF_ERR_CUDA, "cuTensorMapEncodeTiled failed for the decoder's input window");
-      const int64_t tiles = (int64_t)batch * ((H + dec::kTH - 1) / dec::kTH) * ((W + dec::kStrip - 1) / dec::kStrip);
-      const int grid = (int)(tiles < c->sm_count ? tiles : c->sm_count);
-      const size_t smem = sizeof(dec::ConvSmem);
-      if (epi == dec::EPI_RELU) dec::dec_conv7_tma_kernel<dec::EPI_RELU><<<grid, dec::kConvThreads, smem, st>>>(t);
-      else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_tma_kernel<dec::EPI_RES_RELU><<<grid, dec::kConvThreads, smem, st>>>(t);
-      else dec::dec_conv7_tma_kernel<dec::EPI_RES_RELU_RGB><<<grid, dec::kConvThreads, smem, st>>>(t);
-    } else if (impl == 2) {
-      const int64_t tiles = (int64_t)batch * ((H + dec::kTH - 1) / dec::kTH) * ((W + dec::kStrip - 1) / dec::kStrip);
-      const int grid = (int)(tiles < c->sm_count ? tiles : c->sm_count);
-      const size_t smem = sizeof(dec::ConvSmem);
-      if (epi == dec::EPI_RELU) dec::dec_conv7_tc_kernel<dec::EPI_RELU><<<grid, dec::kConvThreads, smem, st>>>(a);
-      else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_tc_kernel<dec::EPI_RES_RELU><<<grid, dec::kConvThreads, smem, st>>>(a);
-      else dec::dec_conv7_tc_kernel<dec::EPI_RES_RELU_RGB><<<grid, dec::kConvThreads, smem, st>>>(a);
-    } else {
-      const unsigned grid = (unsigned)((int64_t)batch * H * ((W + 127) / 128));
-      if (epi == dec::EPI_RELU) dec::dec_conv7_ref_kernel<dec::EPI_RELU><<<grid, 128, 0, st>>>(a);
-      else if (epi == dec::EPI_RES_RELU) dec::dec_conv7_ref_kernel<dec::EPI_RES_RELU><<<grid, 128, 0, st>>>(a);
-      else dec::dec_conv7_ref_kernel<dec::EPI_RES_RELU_RGB><<<grid, 128, 0, st>>>(a);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(B200NERF_ERR_CUDA, cudaGetErrorString(e));
-    return 0;
-  };
   const int H = height, W = width, HO = height * dec::kUp, WO = width * dec::kUp;
-  // rgb_decoder.2, .3: BasicBlocks at feature resolution
-  if (int e = conv(0, dec::EPI_RELU, lo[0], nullptr, lo[1], nullptr, H, W)) return e;
-  if (int e = conv(1, dec::EPI_RES_RELU, lo[1], lo[0], lo[2], nullptr, H, W)) return e;
-  if (int e = conv(2, dec::EPI_RELU, lo[2], nullptr, lo[1], nullptr, H, W)) return e;
-  if (int e = conv(3, dec::EPI_RES_RELU, lo[1], lo[2], lo[0], nullptr, H, W)) return e;
-  // rgb_decoder.4: 3x transposed conv
-  dec::dec_upsample_kernel<<<(unsigned)((lo_px + 2 * dec::kUpThreads - 1) / (2 * dec::kUpThreads)), dec::kUpThreads,
-                             sizeof(float) * (9 * dec::kC * dec::kC + dec::kC), st>>>(
-      lo[0], batch, H, W, d.up_w, d.up_b, hi[0]);
-  CUDA_TRY(cudaGetLastError());
-  // rgb_decoder.5, .6 at image resolution; .7/.8 (1x1 conv + sigmoid) in the last epilogue
-  if (int e = conv(4, dec::EPI_RELU, hi[0], nullptr, hi[1], nullptr, HO, WO)) return e;
-  if (int e = conv(5, dec::EPI_RES_RELU, hi[1], hi[0], hi[2], nullptr, HO, WO)) return e;
-  if (int e = conv(6, dec::EPI_RELU, hi[2], nullptr, hi[1], nullptr, HO, WO)) return e;
-  if (int e = conv(7, dec::EPI_RES_RELU_RGB, hi[1], hi[2], nullptr, rgb, HO, WO)) return e;
+  struct Step {
+    const void* in;
+    const void* res;
+    void* out;
+    int h, w;
+  };
+  const Step steps[10] = {
+      {features, nullptr, lo[0], H, W},  // rgb_decoder.0/.1
+      {lo[0], nullptr, lo[1], H, W}, {lo[1], lo[0], lo[2], H, W},  // rgb_decoder.2
+      {lo[2], nullptr, lo[1], H, W}, {lo[1], lo[2], lo[0], H, W},  // rgb_decoder.3
+      {lo[0], nullptr, hi[0], H, W},                               // rgb_decoder.4 (input resolution)
+      {hi[0], nullptr, hi[1], HO, WO}, {hi[1], hi[0], hi[2], HO, WO},  // rgb_decoder.5
+      {hi[2], nullptr, hi[1], HO, WO}, {hi[1], hi[2], rgb, HO, WO},    // rgb_decoder.6, .7/.8
+  };
+  for (int layer = 0; layer < 10; ++layer) {
+    const Step& s = steps[layer];
+    if (int e = b200nerf_rgb_decode_layer(c, layer, s.in, s.res, s.out, batch, s.h, s.w, impl, stream)) return e;
+  }
   return 0;
 }
 

@@ -9,7 +9,7 @@
 //
 // fp32-level accuracy from bf16 tensor-core inputs: every activation and weight is split into two bf16 numbers
 // (hi = bf16(v), lo = bf16(v - hi)) and each k-step issues three MMAs  a_hi*w_hi + a_lo*w_hi + a_hi*w_lo  into the
-// same accumulator; the dropped a_lo*w_lo term is ~2^-18 relative.  This costs 1.5x the tensor time of a single TF32
+// same accumulator; the dropped a_lo*w_lo term is <= 2^-16 |a||w| (~2^-18 typical).  This costs 1.5x the tensor time of a single TF32
 // pass (bf16 runs at twice the TF32 rate) and needs exactly the bytes of fp32 storage.
 //
 // Activations between layers therefore live in HBM already split ("ACT" layout): per pixel 128 B = 8 chunks of 8 bf16,

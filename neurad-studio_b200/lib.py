@@ -160,6 +160,7 @@ SIGNATURES = {
     "b200nerf_rgb_decode_workspace_bytes": (c_int64, [c_int, c_int, c_int]),
     "b200nerf_rgb_decode_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int64, c_int,
                                         c_void_p]),
+    "b200nerf_rgb_decode_layer": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b200nerf_raygen_pinhole": (c_int, [c_void_p, POINTER(c_float), c_float, c_float, c_float, c_float, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_int, c_int, c_float, POINTER(c_float), c_float,
                                         c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
