@@ -129,11 +129,26 @@ def alpha_weights_backward_matches_float64(dev, n, S, seed=0, be=None):
     w64, ref, T, Rabs = alpha_reference(a, g)
     got = be.alpha_to_weights_bwd(a.to(dev), g.to(dev))
     worst = _ratio(got, ref, alpha_bwd_tol(g, T, Rabs), f"dalpha n={n} S={S}")
-    if dev != "cpu":  # forward: w_i = a_i T_i, a warp-scan product of i factors (any order): <= (2 i + 1) U relative
-        i = torch.arange(S, dtype=torch.float64)
-        tol = (2 * i + 2) * U * w64 + (i + 1) * TINY
-        worst = max(worst, _ratio(be.alpha_to_weights(a.to(dev)), w64, tol, f"alpha weights n={n} S={S}"))
+    if dev != "cpu":
+        worst = max(worst, _ratio(be.alpha_to_weights(a.to(dev)), w64, alpha_weights_forward_tol(w64), f"alpha weights n={n} S={S}"))
     return worst
+
+
+def alpha_weights_forward_tol(w64):
+    """Forward: w_i = a_i T_i, a warp-scan product of i factors (any order): <= (2 i + 1) U relative."""
+    i = torch.arange(w64.shape[1], dtype=torch.float64)
+    return (2 * i + 2) * U * w64 + (i + 1) * TINY
+
+
+def density_weights_forward_tol(delta, dens, w64):
+    """Forward, the terms of E_w in density_bwd_tol (the warp-scan sum of A has the same bound as a sequential one)."""
+    a = delta.double() * dens.double()
+    A = torch.cat([torch.zeros_like(a[:, :1]), torch.cumsum(a, 1)[:, :-1]], 1)
+    i = torch.arange(a.shape[1], dtype=torch.float64)
+    eA, ea = torch.exp(-A), torch.exp(-a)
+    wt = w64.detach()
+    tol = eA * (_mul0(ea, (a + 4) * U) + U * (1 - ea)) + _mul0(wt, _mul0(eA, (i + 1) * U * A + 4 * U) / eA.clamp_min(1e-300) + 2 * U)
+    return torch.nan_to_num(tol, nan=0.0) + 4 * TINY
 
 
 def density_cases(S, n, seed):
@@ -193,15 +208,10 @@ def density_weights_backward_matches_float64(dev, n, S, seed=0, be=None):
     ok = torch.isfinite(ref)
     worst = _ratio(got, ref, density_bwd_tol(delta, dens, g), f"ddensity n={n} S={S}", mask=ok)
     excluded = int((~ok).sum())
-    if dev != "cpu":  # forward, same terms as E_w above (the warp-scan sum of A has the same bound as a sequential one)
-        a = delta.double() * dens.double()
-        A = torch.cat([torch.zeros_like(a[:, :1]), torch.cumsum(a, 1)[:, :-1]], 1)
-        i = torch.arange(S, dtype=torch.float64)
-        eA, ea = torch.exp(-A), torch.exp(-a)
+    if dev != "cpu":
         wt = w64.detach()
-        tol = eA * (_mul0(ea, (a + 4) * U) + U * (1 - ea)) + _mul0(wt, _mul0(eA, (i + 1) * U * A + 4 * U) / eA.clamp_min(1e-300) + 2 * U)
-        tol = torch.nan_to_num(tol, nan=0.0) + 4 * TINY
-        worst = max(worst, _ratio(be.density_to_weights(delta.to(dev), dens.to(dev)), wt, tol, f"density weights n={n} S={S}"))
+        worst = max(worst, _ratio(be.density_to_weights(delta.to(dev), dens.to(dev)), wt, density_weights_forward_tol(delta, dens, wt),
+                                  f"density weights n={n} S={S}"))
     return worst, excluded
 
 
