@@ -353,18 +353,28 @@ constexpr int kLanePanelRows = kGeoIn + kSh + 1;  // grid features | SH | sdf
 constexpr size_t lane_tc_smem_bytes() { return (size_t)kTcBytes + sizeof(float) * kLanePanelRows * kLanePanelPitch; }
 struct MlpLaneTc {
   static constexpr int kPitch = kLanePanelPitch;
-  const TcShared* t;  // B tiles staged by tc_stage_weights(..., chained = true)
+  const TcShared* t;  // B tiles staged by tc_stage_weights(..., chained = true); at the start of dynamic shared memory
   float* panel_;      // [kLanePanelRows][kPitch] shared memory
   int bar_id;         // this warp group's named barrier
   int sh_tcnn = 0;    // 1: tiny-cuda-nn's SphericalHarmonics convention
   NFF_D float* panel() const { return panel_; }
   NFF_D void group_sync() const { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); }
 
+  // Low descriptor word (tc::smem_desc_lo, LBO 128 B) of t->b, taken from the dynamic shared memory symbol rather than
+  // from `t`: ptxas then computes it, and every descriptor derived from it, on the uniform datapath.  From the generic
+  // pointer it built all 66 descriptors of a half in per-thread registers and moved each into a uniform register pair
+  // (two R2UR per wgmma; one R2UR per half is left, DESIGN section 4).
+  NFF_D static uint32_t b_desc_lo() {
+    extern __shared__ __align__(128) unsigned char nff_lane_smem[];  // = the kernel's dynamic shared memory
+    return tc::smem_desc_lo(tc::smem_u32(nff_lane_smem + offsetof(TcShared, b)), 128u);
+  }
+
   // acc (this thread's 16 fragment registers of one m64n32 half, preset by the caller) += A * W^T over KS k-steps of a
-  // layer with K inputs, 3xTF32; a = the A fragments, 4 per k-step; b_hi = the layer's hi B tile (lo follows it) from
-  // its first k-step on (tc::b_elem_offset: one k-step is 64 floats).
-  template <int KS, int K>
-  NFF_D static void half_mma(float* acc, const float* a, const float* b_hi) {
+  // layer with K inputs, 3xTF32; a = the A fragments, 4 per k-step; OFF = the float offset in t->b of the layer's hi B
+  // tile (lo follows it) from its first k-step on (tc::b_elem_offset: one k-step is 64 floats).  Every descriptor is
+  // b_desc_lo() plus a compile-time constant.
+  template <int KS, int K, int OFF>
+  NFF_D static void half_mma(float* acc, const float* a) {
     uint32_t ah[4 * KS], al[4 * KS];
 #pragma unroll
     for (int i = 0; i < 4 * KS; ++i) {
@@ -372,15 +382,17 @@ struct MlpLaneTc {
       ah[i] = __float_as_uint(h);
       al[i] = __float_as_uint(a[i] - h);
     }
-    const uint32_t sbo = (uint32_t)(K / 4) * 128u;  // (K / 4) core matrices of 128 B per 8-row n block
-    const uint64_t dh = tc::smem_desc(tc::smem_u32(b_hi), 128u, sbo), dl = tc::smem_desc(tc::smem_u32(b_hi + 32 * K), 128u, sbo);
+    constexpr uint32_t sbo = (uint32_t)(K / 4) * 128u;  // (K / 4) core matrices of 128 B per 8-row n block
+    constexpr uint32_t hi_off = (uint32_t)OFF * 4u / 16u, lo_off = (uint32_t)(OFF + 32 * K) * 4u / 16u;
+    const uint32_t b_desc = b_desc_lo();
     tc::wg_fence();
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
-      const uint64_t adv = (uint64_t)((ks * 2 * 128) >> 4);  // two 16-byte K-chunks per k-step
-      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dh + adv);
-      tc::wgmma_tf32<32>(acc, al + 4 * ks, dh + adv);
-      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dl + adv);
+      const uint32_t adv = (uint32_t)(ks * 2 * 128) / 16u;  // two 16-byte K-chunks per k-step
+      const uint64_t dh = tc::smem_desc_of(b_desc + hi_off + adv, sbo), dl = tc::smem_desc_of(b_desc + lo_off + adv, sbo);
+      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dh);
+      tc::wgmma_tf32<32>(acc, al + 4 * ks, dh);
+      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dl);
     }
     tc::wg_commit();
     tc::wg_wait<0>();
@@ -442,7 +454,7 @@ struct MlpLaneTc {
       // layer 0: grid features -> hidden, ReLU, sdf
       load_a(a, p, q, 0, 4);
       bias_init(acc, t->bias[0], q);
-      half_mma<4, 32>(acc, a, t->b + tc_layer_off(0));
+      half_mma<4, 32, tc_layer_off(0)>(acc, a);
       relu(acc);
       float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
@@ -462,7 +474,7 @@ struct MlpLaneTc {
       // layer 1: -> geo_embedding, parked at this thread's fragment positions of panel rows 0..31
       chain(a, acc);
       bias_init(acc, t->bias[1], q);
-      half_mma<4, 32>(acc, a, t->b + tc_layer_off(1));
+      half_mma<4, 32, tc_layer_off(1)>(acc, a);
       __syncwarp();  // the warp's layer-0 fragment loads of these rows are done
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -472,14 +484,14 @@ struct MlpLaneTc {
       // layer 2: [geo_embedding | SH] -> hidden, ReLU
       chain(a, acc);
       bias_init(acc, t->bias[2], q);
-      half_mma<4, 48>(acc, a, t->b + tc_layer_off(2));
+      half_mma<4, 48, tc_layer_off(2)>(acc, a);
       load_a(a, p, q, 4, 2);
-      half_mma<2, 48>(acc, a, t->b + tc_layer_off(2) + 4 * 64);
+      half_mma<2, 48, tc_layer_off(2) + 4 * 64>(acc, a);
       relu(acc);
       // layer 3: hidden -> hidden, ReLU
       chain(a, acc);
       bias_init(acc, t->bias[3], q);
-      half_mma<4, 32>(acc, a, t->b + tc_layer_off(3));
+      half_mma<4, 32, tc_layer_off(3)>(acc, a);
       relu(acc);
       // layer 4: hidden -> features, accumulated onto bias + geo_embedding; out to the same positions
       chain(a, acc);
@@ -489,7 +501,7 @@ struct MlpLaneTc {
         const float* r = p + (8 * j + 2 * q) * kPitch;
         acc[4 * j + 0] += r[0], acc[4 * j + 1] += r[kPitch], acc[4 * j + 2] += r[8], acc[4 * j + 3] += r[kPitch + 8];
       }
-      half_mma<4, 32>(acc, a, t->b + tc_layer_off(4));
+      half_mma<4, 32, tc_layer_off(4)>(acc, a);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         float* r = p + (8 * j + 2 * q) * kPitch;

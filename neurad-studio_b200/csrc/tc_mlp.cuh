@@ -153,6 +153,17 @@ __device__ __forceinline__ void stage_b_tile(float* hi, float* lo, const float* 
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
+// The same descriptor as two 32-bit words: lo = start and LBO fields, hi = SBO field.  A tile `off` bytes further on has
+// lo + off / 16 (the start field cannot carry into the LBO field: shared memory ends below 2^18 bytes), so every
+// descriptor of a CTA's resident B tiles is one lo word plus compile-time constants.  When that word comes from a shared
+// memory symbol, ptxas forms the descriptors on the uniform datapath: no per-thread descriptor arithmetic and no R2UR
+// move in front of each wgmma.
+__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
+  return ((saddr & 0x3ffffu) >> 4) | ((lbo_bytes >> 4) << 16);
+}
+__device__ __forceinline__ uint64_t smem_desc_of(uint32_t lo, uint32_t sbo_bytes) {
+  return (uint64_t)lo | ((uint64_t)(sbo_bytes >> 4) << 32);
+}
 
 // ------------------------------------------------------------------------------------------------ tile ops
 // Row pitch (floats) of a 128-row stage holding up to W columns.
