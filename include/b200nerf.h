@@ -21,6 +21,7 @@
 #ifndef B200NERF_H_
 #define B200NERF_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -602,6 +603,40 @@ int b200nerf_raygen_lidar_grid(b200nerf_ctx* ctx, const float* l2w_host, float e
 int b200nerf_chamfer_distance(b200nerf_ctx* ctx, const float* src, int64_t n_src, int src_stride, const float* dst,
                               int64_t n_dst, int dst_stride, int normalize_by_dst, double* out_scalar, float* min_src,
                               float* min_dst, void* stream);
+
+/* ---- lidar training losses ------------------------------------------------------------------------------ */
+
+/* The lidar terms of NeuRADModel.get_metrics_dict in training mode (models/neurad.py:486-520) over the n lidar rays of a
+ * batch.  Every per-ray array is in LIDAR ROWS (the rays whose is_lidar is set, in batch order), fp32 unless noted:
+ * pred [n] (outputs["depth"][is_lidar]), prop [n_prop][prop_stride] (the proposal depths), distance [n], did_return [n]
+ * (uint8), intensity [n] (predicted), gt_intensity [n] with row stride gt_intensity_stride (column 3 of batch["lidar"]),
+ * logits [n] (ray-drop logits).
+ *
+ * out (device, fp32) = [depth_loss, intensity_loss, ray_drop_loss, quantile, depth_loss_0 .. depth_loss_{n_prop-1}]:
+ * the quantile is torch.quantile(loss, quantile) bit for bit (NaN if any loss is NaN), mask [n] (uint8) = loss <
+ * quantile, counts (device, int32) = [|mask|, |mask & did_return|].  Sums are fp64 in a fixed order (bit-reproducible);
+ * a mean over an empty mask is NaN.  No host synchronisation.  1 <= n <= 2^24 (torch.quantile's limit), n_prop <= 4 and
+ * strides below 2^31 are checked on the host; workspace holds at least b200nerf_lidar_losses_workspace_bytes(n) bytes. */
+size_t b200nerf_lidar_losses_workspace_bytes(int64_t n);
+int b200nerf_lidar_losses_fwd(b200nerf_ctx* ctx, int64_t n, int n_prop, const float* pred, const float* prop,
+                              int64_t prop_stride, const float* distance, const uint8_t* did_return, const float* intensity,
+                              const float* gt_intensity, int64_t gt_intensity_stride, const float* logits,
+                              float non_return_distance, float non_return_mult, float quantile, float* out, int* counts,
+                              uint8_t* mask, void* workspace, size_t workspace_bytes, void* stream);
+/* Gradients of the forward's scalars with respect to pred, prop ([n_prop][n], dense), intensity and logits, for upstream
+ * gradients grads (device, fp32) in the layout of the forward's `out` (the quantile's entry is not read); mask and
+ * counts are the forward's.  No gradient flows through the mask or the non-return targets. */
+int b200nerf_lidar_losses_bwd(b200nerf_ctx* ctx, int64_t n, int n_prop, const float* pred, const float* prop,
+                              int64_t prop_stride, const float* distance, const uint8_t* did_return, const float* intensity,
+                              const float* gt_intensity, int64_t gt_intensity_stride, const float* logits,
+                              float non_return_distance, float non_return_mult, const uint8_t* mask, const int* counts,
+                              const float* grads, float* d_pred, float* d_prop, float* d_intensity, float* d_logits,
+                              void* stream);
+/* The order statistic of the forward on its own: *out (device) = torch.quantile(x, q) (linear interpolation), or with
+ * lower_median torch.median(x), bit for bit, for x [n] fp32 and 1 <= n <= 2^24; workspace as for n = 0.  One exception:
+ * -0 and +0 are one key, so a zero at the rank comes back as +0 where torch's sort may leave a -0 there. */
+int b200nerf_quantile(b200nerf_ctx* ctx, const float* x, int64_t n, float q, int lower_median, float* out, void* workspace,
+                      size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -35,6 +35,12 @@ import neurad_studio_b200 as nsb
 from neurad_studio_b200 import nerfstudio_api as _api
 
 
+# LossSettings fields carried flat by NeuRADConfig (neurad.py:66-94), besides carving_epsilon,
+# non_return_lidar_distance and ray_drop_loss_mult
+LOSS_SETTINGS = ("rgb_mult", "vgg_mult", "depth_mult", "intensity_mult", "carving_mult", "quantile_threshold",
+                 "interlevel_loss_mult", "distortion_loss_mult", "non_return_loss_mult", "prop_lidar_loss_mult")
+
+
 def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
     """The numbers of the reference model's config tree that shape the path (neurad.py:97-162, neurad_field.py:44-75,
     155-182, neurad_encoding.py:34-82) as the backend's flat config."""
@@ -65,6 +71,7 @@ def config_from_reference(model: NeuRADModel) -> nsb.NeuRADConfig:
         rgb_hidden_dim=mc.rgb_hidden_dim, actor_bbox_padding=tuple(mc.dynamic_actors.actor_bbox_padding),
         static_scale=float(model.scene_box.aabb.max()), duration=float(model._duration), num_sensors=num_sensors,
         n_actors=int(model.dynamic_actors.n_actors), ray_drop_loss_mult=float(mc.loss.ray_drop_loss_mult),
+        **{k: float(getattr(mc.loss, k)) for k in LOSS_SETTINGS},
     )
 
 

@@ -300,6 +300,31 @@ class InterlevelLossFn(Function):
         return None, None, None, None, dwp * dloss[:, None], None
 
 
+class LidarLossesFn(Function):
+    """The lidar terms of get_metrics_dict in training mode (neurad.py:486-520) over the lidar rows: out [4 + rounds] =
+    [depth_loss, intensity_loss, ray_drop_loss, quantile, depth_loss_0, ...] and the quantile mask.  Gradients go to the
+    predicted depth, the proposal depths, the intensity and the ray-drop logits; none flows through the mask, the quantile
+    or the non-return targets.  `settings` = (non_return_lidar_distance, non_return_loss_mult, quantile_threshold)."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, be, settings, distance, did_return, gt_intensity, pred, intensity, logits, *prop):
+        out, counts, mask = be.lidar_losses(pred, prop, distance, did_return, intensity, gt_intensity, logits, *settings)
+        ctx.be, ctx.settings = be, settings
+        ctx.save_for_backward(distance, did_return, gt_intensity, pred, intensity, logits, mask, counts, *prop)
+        ctx.mark_non_differentiable(mask)
+        return out, mask
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, d_out, _d_mask):
+        distance, did_return, gt, pred, intensity, logits, mask, counts, *prop = ctx.saved_tensors
+        dp, dprop, di, dl = ctx.be.lidar_losses_bwd(pred, prop, distance, did_return, intensity, gt, logits, *ctx.settings[:2],
+                                                    mask, counts, d_out)
+        return (None, None, None, None, None, dp.view(pred.shape), di.view(intensity.shape), dl.view(logits.shape),
+                *(dprop[i].view(p.shape) for i, p in enumerate(prop)))
+
+
 class HashGridFn(Function):
     """HashEncoding.forward (the stand-alone grid, encodings.py:425-471): gradient to the hash table (the reference also
     differentiates with respect to the positions; NeuRAD's path never asks for that on a stand-alone grid -- its position

@@ -986,3 +986,72 @@ class B200Backend:
                                                        int(bool(normalize_with_target)), _ptr(out), _ptr(min_p), _ptr(min_g),
                                                        self._stream))
         return (out, min_p, min_g) if want_minima else out
+
+    # ------------------------------------------------------------------------------------------ lidar training losses
+    def _lidar_loss_rows(self, pred, prop, distance, did_return, intensity, gt_intensity, logits):
+        """Flatten the lidar-row inputs of the lidar losses to what the C ABI takes (no host synchronisation)."""
+        def row(t):
+            return self._dev(t.reshape(-1))
+
+        n = distance.numel()
+        gt = gt_intensity.detach().reshape(-1)
+        if gt.device != self.device or gt.dtype != torch.float32:
+            gt = self._dev(gt)
+        p = [row(t) for t in prop]
+        p = torch.stack(p) if p else None
+        ret = did_return.detach().reshape(-1).to(device=self.device, dtype=torch.uint8)
+        rows = (row(pred), p, row(distance), ret, row(intensity), gt, row(logits))
+        if any(t is not None and t.shape[-1] != n for t in rows):
+            raise ValueError("lidar losses: every per-ray input needs one entry per lidar ray")
+        return rows
+
+    def lidar_losses(self, pred, prop, distance, did_return, intensity, gt_intensity, logits, non_return_distance: float,
+                     non_return_mult: float, quantile: float):
+        """The lidar terms of get_metrics_dict in training mode (neurad.py:486-520) over n lidar rays.  Every input is in
+        lidar rows ([n] or [n,1]): predicted depth, a list of proposal depths, measured distance, did_return (bool),
+        predicted intensity, measured intensity (a strided column such as `lidar[:, 3]` is fine) and ray-drop logits.
+
+        Returns (out, counts, mask): out [4 + rounds] fp32 = [depth_loss, intensity_loss, ray_drop_loss, quantile,
+        depth_loss_0, ...], counts [2] int32 = [|mask|, |mask & did_return|], mask [n] bool = loss < quantile.  Nothing
+        synchronises the host; n = 0 raises (torch.quantile of an empty tensor does too)."""
+        n = distance.numel()
+        if n == 0:
+            raise _lib.B200NerfError("lidar losses of a batch without lidar rays (torch.quantile of an empty tensor)")
+        pr, pp, d, ret, it, gt, lg = self._lidar_loss_rows(pred, prop, distance, did_return, intensity, gt_intensity, logits)
+        r = 0 if pp is None else pp.shape[0]
+        out = torch.empty(4 + r, device=self.device)
+        counts = torch.empty(2, dtype=torch.int32, device=self.device)
+        mask = torch.empty(n, dtype=torch.bool, device=self.device)
+        ws = torch.empty(int(self.lib.b200nerf_lidar_losses_workspace_bytes(n)), dtype=torch.uint8, device=self.device)
+        self._check(self.lib.b200nerf_lidar_losses_fwd(
+            self._h, n, r, _ptr(pr), _ptr(pp), n, _ptr(d), _ptr(ret), _ptr(it), _ptr(gt), gt.stride(0), _ptr(lg),
+            float(non_return_distance), float(non_return_mult), float(quantile), _ptr(out), _ptr(counts), _ptr(mask),
+            _ptr(ws), ws.numel(), self._stream))
+        return out, counts, mask
+
+    def lidar_losses_bwd(self, pred, prop, distance, did_return, intensity, gt_intensity, logits, non_return_distance: float,
+                         non_return_mult: float, mask, counts, grad_out):
+        """Gradients of `lidar_losses`' out for upstream gradients grad_out [4 + rounds] (device; the quantile's entry is
+        not read): (d pred [n], d prop [rounds, n], d intensity [n], d logits [n]).  mask / counts are the forward's."""
+        n = distance.numel()
+        pr, pp, d, ret, it, gt, lg = self._lidar_loss_rows(pred, prop, distance, did_return, intensity, gt_intensity, logits)
+        r = 0 if pp is None else pp.shape[0]
+        g = self._dev(grad_out)
+        d_pred, d_int, d_lg = (torch.empty(n, device=self.device) for _ in range(3))
+        d_prop = torch.empty(r, n, device=self.device)
+        self._check(self.lib.b200nerf_lidar_losses_bwd(
+            self._h, n, r, _ptr(pr), _ptr(pp), n, _ptr(d), _ptr(ret), _ptr(it), _ptr(gt), gt.stride(0), _ptr(lg),
+            float(non_return_distance), float(non_return_mult), _ptr(mask), _ptr(counts), _ptr(g), _ptr(d_pred),
+            _ptr(d_prop) if r else None, _ptr(d_int), _ptr(d_lg), self._stream))
+        return d_pred, d_prop, d_int, d_lg
+
+    def quantile(self, x: torch.Tensor, q: float, lower_median: bool = False) -> torch.Tensor:
+        """torch.quantile(x, q) (linear interpolation), or with `lower_median` torch.median(x), over all of x, bit for bit,
+        as a 0-d device tensor and without a host synchronisation; the selection of `lidar_losses`.  1 <= x.numel() <= 2^24.
+        -0 and +0 are one key: a zero at the rank comes back as +0 (torch may return -0 there)."""
+        v = self._dev(x.reshape(-1))
+        out = torch.empty((), device=self.device)
+        ws = torch.empty(int(self.lib.b200nerf_lidar_losses_workspace_bytes(0)), dtype=torch.uint8, device=self.device)
+        self._check(self.lib.b200nerf_quantile(self._h, _ptr(v), v.numel(), float(q), int(bool(lower_median)), _ptr(out),
+                                               _ptr(ws), ws.numel(), self._stream))
+        return out

@@ -113,6 +113,18 @@ class NeuRADConfig:
     # LossSettings.ray_drop_loss_mult (neurad.py:91); the lidar metrics' predicted returns are ray-drop probabilities < 0.5
     # when it is > 0, depths < non_return_lidar_distance otherwise (neurad.py:610-613)
     ray_drop_loss_mult: float = 0.01
+    # the rest of LossSettings (neurad.py:66-94), flat, with the reference's defaults: the multipliers and the lidar
+    # depth loss's quantile of NeuRADModel.get_metrics_dict / get_loss_dict (neurad.py:461-561)
+    rgb_mult: float = 5.0
+    vgg_mult: float = 0.05
+    depth_mult: float = 0.01
+    intensity_mult: float = 0.1
+    carving_mult: float = 0.01
+    quantile_threshold: float = 0.95
+    interlevel_loss_mult: float = 0.001
+    distortion_loss_mult: float = 0.002
+    non_return_loss_mult: float = 0.1
+    prop_lidar_loss_mult: float = 0.1
     # scene-level constants (dataset metadata in the reference)
     static_scale: float = 100.0
     duration: float = 8.0

@@ -13,6 +13,7 @@
 #include "rgb_decoder.cuh"
 #include "modules.cuh"
 #include "lidar_eval.cuh"
+#include "lidar_loss.cuh"
 
 using namespace nff;
 
@@ -2479,6 +2480,109 @@ int b200nerf_chamfer_distance(b200nerf_ctx* c, const float* src, int64_t n_src, 
   chamfer_reduce_kernel<<<1, kChamferReduceThreads, 0, s>>>(reinterpret_cast<unsigned*>(min_src), (int)n_src,
                                                             reinterpret_cast<unsigned*>(min_dst), (int)n_dst,
                                                             normalize_by_dst, out_scalar);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---- lidar training losses (lidar_loss.cuh)
+static const size_t kLossStateBytes = sizeof(SelectState) + sizeof(unsigned) * kSelectBins;
+static const size_t kLossHeaderBytes =
+    kLossStateBytes + sizeof(double) * kLossMaxBlocks * (kRowSlots + kMaskSlots);
+static int loss_blocks(int64_t n) {
+  const int64_t b = (n + kLossThreads - 1) / kLossThreads;
+  return (int)(b < 1 ? 1 : b > kLossMaxBlocks ? kLossMaxBlocks : b);
+}
+
+size_t b200nerf_lidar_losses_workspace_bytes(int64_t n) { return kLossHeaderBytes + sizeof(float) * (size_t)(n > 0 ? n : 0); }
+
+// Passes 1 and 2 of the selection (pass 0's histogram is already in `hist`), the ceil statistic and the value.
+static void select_rest(const float* vals, int n, float q, int lower_median, SelectState* st, unsigned* hist, float* out,
+                        cudaStream_t s) {
+  const int blocks = loss_blocks(n);
+  for (int pass = 0; pass < kSelectPasses; ++pass) {
+    if (pass > 0) select_hist_kernel<<<blocks, kLossThreads, 0, s>>>(vals, n, pass, st, hist);
+    select_scan_kernel<<<1, 1024, 0, s>>>(n, q, lower_median, pass, st, hist);
+  }
+  select_above_kernel<<<blocks, kLossThreads, 0, s>>>(vals, n, st);
+  select_finish_kernel<<<1, 1, 0, s>>>(st, out);
+}
+
+int b200nerf_lidar_losses_fwd(b200nerf_ctx* c, int64_t n, int n_prop, const float* pred, const float* prop,
+                              int64_t prop_stride, const float* distance, const uint8_t* did_return, const float* intensity,
+                              const float* gt_intensity, int64_t gt_intensity_stride, const float* logits,
+                              float non_return_distance, float non_return_mult, float quantile, float* out, int* counts,
+                              uint8_t* mask, void* workspace, size_t workspace_bytes, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n >= 1, "lidar losses of an empty batch (torch.quantile of an empty tensor)");
+  REQUIRE(n <= kLossMaxN, "lidar losses support at most 2^24 rays (torch.quantile's limit)");
+  REQUIRE(n_prop >= 0 && n_prop <= kLossMaxProp, "at most 4 proposal rounds");
+  REQUIRE(n_prop == 0 || (prop && prop_stride >= n), "proposal depths missing or overlapping");
+  REQUIRE(gt_intensity_stride >= 1 && gt_intensity_stride <= 0x7fffffff, "intensity stride must be in [1, 2^31 - 1]");
+  REQUIRE(prop_stride <= 0x7fffffff, "proposal-depth stride must be below 2^31");
+  REQUIRE(pred && distance && did_return && intensity && gt_intensity && logits && out && counts && mask, "NULL argument");
+  REQUIRE(workspace && workspace_bytes >= b200nerf_lidar_losses_workspace_bytes(n), "workspace too small");
+  DeviceGuard g(c->device);
+  const cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  SelectState* st = (SelectState*)ws;
+  unsigned* hist = (unsigned*)(ws + sizeof(SelectState));
+  double* row_part = (double*)(ws + kLossStateBytes);
+  double* mask_part = row_part + kLossMaxBlocks * kRowSlots;
+  float* loss = (float*)(ws + kLossHeaderBytes);
+  const LidarLossArgs a{(int)n, n_prop, (int)prop_stride, (int)gt_intensity_stride, pred, prop, distance, did_return,
+                        intensity, gt_intensity, logits, non_return_distance, non_return_mult};
+  const int blocks = loss_blocks(n);
+  CUDA_TRY(cudaMemsetAsync(ws, 0, kLossStateBytes, s));
+  lidar_loss_rows_kernel<<<blocks, kLossThreads, 0, s>>>(a, loss, st, hist, row_part);
+  select_rest(loss, (int)n, quantile, 0, st, hist, nullptr, s);
+  lidar_loss_mask_kernel<<<blocks, kLossThreads, 0, s>>>(a, loss, st, mask, mask_part);
+  lidar_loss_final_kernel<<<1, 32, 0, s>>>((int)n, n_prop, blocks, row_part, mask_part, st, out, counts);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b200nerf_lidar_losses_bwd(b200nerf_ctx* c, int64_t n, int n_prop, const float* pred, const float* prop,
+                              int64_t prop_stride, const float* distance, const uint8_t* did_return, const float* intensity,
+                              const float* gt_intensity, int64_t gt_intensity_stride, const float* logits,
+                              float non_return_distance, float non_return_mult, const uint8_t* mask, const int* counts,
+                              const float* grads, float* d_pred, float* d_prop, float* d_intensity, float* d_logits,
+                              void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n >= 1 && n <= kLossMaxN, "lidar losses support 1 to 2^24 rays");
+  REQUIRE(n_prop >= 0 && n_prop <= kLossMaxProp, "at most 4 proposal rounds");
+  REQUIRE(n_prop == 0 || (prop && prop_stride >= n && d_prop), "proposal depths missing or overlapping");
+  REQUIRE(gt_intensity_stride >= 1 && gt_intensity_stride <= 0x7fffffff, "intensity stride must be in [1, 2^31 - 1]");
+  REQUIRE(prop_stride <= 0x7fffffff, "proposal-depth stride must be below 2^31");
+  REQUIRE(pred && distance && did_return && intensity && gt_intensity && logits && mask && counts && grads && d_pred &&
+              d_intensity && d_logits,
+          "NULL argument");
+  DeviceGuard g(c->device);
+  const LidarLossArgs a{(int)n, n_prop, (int)prop_stride, (int)gt_intensity_stride, pred, prop, distance, did_return,
+                        intensity, gt_intensity, logits, non_return_distance, non_return_mult};
+  const int64_t want = (n + kLossThreads - 1) / kLossThreads;
+  const int blocks = (int)(want < (int64_t)c->sm_count * 8 ? want : (int64_t)c->sm_count * 8);
+  lidar_loss_bwd_kernel<<<blocks, kLossThreads, 0, (cudaStream_t)stream>>>(a, mask, counts, grads, d_pred, d_prop, d_intensity,
+                                                                            d_logits);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b200nerf_quantile(b200nerf_ctx* c, const float* x, int64_t n, float q, int lower_median, float* out, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n >= 1, "quantile of an empty tensor");
+  REQUIRE(n <= kLossMaxN, "quantile supports at most 2^24 values (torch.quantile's limit)");
+  REQUIRE(lower_median || (q >= 0.f && q <= 1.f), "q must be in [0, 1]");
+  REQUIRE(x && out, "NULL argument");
+  REQUIRE(workspace && workspace_bytes >= b200nerf_lidar_losses_workspace_bytes(0), "workspace too small");
+  DeviceGuard g(c->device);
+  const cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  SelectState* st = (SelectState*)ws;
+  unsigned* hist = (unsigned*)(ws + sizeof(SelectState));
+  CUDA_TRY(cudaMemsetAsync(ws, 0, kLossStateBytes, s));
+  select_hist_kernel<<<loss_blocks(n), kLossThreads, 0, s>>>(x, (int)n, 0, st, hist);
+  select_rest(x, (int)n, q, lower_median, st, hist, out, s);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -4,7 +4,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint8, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint8, c_void_p
 
 from . import build as _build
 
@@ -172,6 +172,14 @@ SIGNATURES = {
                                              c_void_p, c_void_p, c_void_p]),
     "b200nerf_chamfer_distance": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int64, c_int, c_int, c_void_p,
                                           c_void_p, c_void_p, c_void_p]),
+    "b200nerf_lidar_losses_workspace_bytes": (c_size_t, [c_int64]),
+    "b200nerf_lidar_losses_fwd": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_int64, c_void_p, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_size_t, c_void_p]),
+    "b200nerf_lidar_losses_bwd": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_int64, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200nerf_quantile": (c_int, [c_void_p, c_void_p, c_int64, c_float, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 _LIB = None

@@ -1,4 +1,4 @@
-"""NeuRAD's lidar evaluation metrics (models/neurad.py:268-271, 589-621).
+"""NeuRAD's lidar evaluation metrics (models/neurad.py:268-271, 589-621) and the training PSNR of get_metrics_dict.
 
 `chamfer_distance` is the reference's `nerfstudio.utils.math.chamfer_distance` on the library's all-pairs kernel
 (csrc/lidar_eval.cuh): exact fp32 per-pair squared distances from direct differences and fp64 sums, without the dense
@@ -7,6 +7,7 @@ reference.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -44,3 +45,8 @@ def mean_rel_l2(pred: Tensor, gt: Tensor) -> Tensor:
 
 def rmse(pred: Tensor, gt: Tensor) -> Tensor:
     return torch.sqrt(torch.mean((pred - gt) ** 2))
+
+
+def psnr(preds: Tensor, target: Tensor) -> Tensor:
+    """torchmetrics' PeakSignalNoiseRatio(data_range=1.0) on one batch (neurad.py:265, 465): 10 log10(1 / mse)."""
+    return -torch.log(torch.sum((preds - target) ** 2) / target.numel()) * (10 / math.log(10.0))

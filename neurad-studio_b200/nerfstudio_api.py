@@ -1071,6 +1071,9 @@ class NeuRADModel(nn.Module):
         # lidar metrics (neurad.py:268-271); the chamfer distance runs on the library's all-pairs kernel
         self.median_l2, self.mean_rel_l2, self.rmse = M.median_l2, M.mean_rel_l2, M.rmse
         self.chamfer_distance = lambda pred, gt: M.chamfer_distance(pred, gt, 1_000, True)
+        # get_loss_dict's perceptual term (neurad.py:260, 537-538): any callable (rgb, image) -> loss, e.g. the reference's
+        # VGGPerceptualLossPix2Pix.  The library ships no VGG19 weights, so it is None until the caller assigns one.
+        self.vgg_loss = None
 
     # -- nn.Module state dict in the reference's key format --------------------------------------------------------
     @staticmethod
@@ -1407,6 +1410,94 @@ class NeuRADModel(nn.Module):
         pts = ray_bundle.origins + ray_bundle.directions * outputs["depth"]
         outputs["points"] = pts @ rot_t.t() - (rot_t @ l2w[:3, 3])
         return outputs, batch
+
+    # -- training objective ---------------------------------------------------------------------------------------
+    def get_metrics_dict(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor]) -> Dict[str, Tensor]:
+        """neurad.py:461-529 with the reference's keys and conditions.  Image batches: psnr.  Lidar batches: the four eval
+        metrics (the reference's boolean-mask gathers) and, in training mode, the lidar losses on the library's kernels
+        (losses.lidar_losses: depth with the non-return targets and the exact 0.95-quantile mask, intensity, ray drop,
+        the per-round proposal depths; no host synchronisation) and the carving sums.  Training with `weights_list`:
+        distortion.  Always: sdf_to_density and the camera optimizer's metrics.
+
+        The batch is the reference's: is_lidar / did_return [N,1] over all rays, distance [n,1] and lidar [n,>=4] over the
+        lidar rays; the outputs those of get_outputs (intensity and ray_drop_logits in lidar rows)."""
+        from . import losses as L
+
+        device = self.static_scale.device
+        cfg = self.config
+        metrics_dict: Dict[str, Tensor] = {}
+        if "image" in batch:
+            image, rgb = batch["image"].to(device), outputs["rgb"]
+            metrics_dict["psnr"] = M.psnr(rgb.detach(), image)
+        if "lidar" in batch:
+            is_lidar = batch["is_lidar"][:, 0].to(device)
+            n_lidar_rays = is_lidar.sum()
+            did_return = batch["did_return"][batch["is_lidar"].squeeze(-1)].squeeze(-1).to(device)
+            points_intensities = batch["lidar"][..., 3:4].to(device)
+            termination_depth = batch["distance"].to(device)
+            pred_depth = outputs["depth"][is_lidar]
+            ray_drop_logits = outputs["ray_drop_logits"]
+            pred_intensity = outputs["intensity"]
+
+            metrics_dict["depth_median_l2"] = self.median_l2(pred_depth[did_return], termination_depth[did_return])
+            metrics_dict["depth_mean_rel_l2"] = self.mean_rel_l2(pred_depth[did_return], termination_depth[did_return])
+            metrics_dict["intensity_rmse"] = self.rmse(pred_intensity[did_return], points_intensities[did_return])
+            metrics_dict["ray_drop_accuracy"] = ((ray_drop_logits.sigmoid() > 0.5).squeeze(-1) == ~did_return).float().mean()
+
+            if self.training:
+                rounds = len(cfg.sampling.num_proposal_samples)
+                lidar = L.lidar_losses(pred_depth, [outputs[f"prop_depth_{i}"][is_lidar] for i in range(rounds)],
+                                       termination_depth, did_return, pred_intensity, points_intensities, ray_drop_logits,
+                                       cfg.non_return_lidar_distance, cfg.non_return_loss_mult, cfg.quantile_threshold)
+                for k in ("depth_loss", "intensity_loss", "ray_drop_loss"):
+                    metrics_dict[k] = lidar[k]
+                metrics_dict["carving_loss"] = (outputs["non_nearby_weights"] ** 2).sum() / n_lidar_rays
+                for i in range(rounds):
+                    metrics_dict[f"depth_loss_{i}"] = lidar[f"depth_loss_{i}"]
+                    metrics_dict[f"carving_loss_{i}"] = outputs[f"prop_weights_loss_{i}"] / n_lidar_rays
+
+        if self.training and "weights_list" in outputs:
+            metrics_dict["distortion"] = L.distortion_loss(outputs["weights_list"], outputs["ray_samples_list"])
+        metrics_dict["sdf_to_density"] = float(self._param("field.sdf_to_density.beta").detach())  # NeuRAD's field is an SDF
+        self.camera_optimizer.get_metrics_dict(metrics_dict)
+        return metrics_dict
+
+    def get_loss_dict(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor],
+                      metrics_dict: Optional[Dict[str, Tensor]] = None) -> Dict[str, Tensor]:
+        """neurad.py:531-561 with the reference's keys, multipliers and conditions.  An image batch with vgg_mult > 0
+        needs `self.vgg_loss` (see __init__): without it this raises rather than return a loss dict without the
+        perceptual term."""
+        from . import losses as L
+
+        cfg = self.config
+        loss_dict: Dict[str, Tensor] = {}
+        if "image" in batch:
+            image, rgb = batch["image"].to(self.static_scale.device), outputs["rgb"]
+            if cfg.vgg_mult > 0.0 and self.vgg_loss is None:
+                raise RuntimeError("vgg_mult > 0 needs a perceptual loss: assign model.vgg_loss = a callable (rgb, image) -> "
+                                   "loss (e.g. the reference's VGGPerceptualLossPix2Pix; no VGG weights ship with "
+                                   "neurad_studio_b200) or set vgg_mult = 0")
+            loss_dict["rgb_loss"] = torch.nn.functional.mse_loss(image, rgb) * cfg.rgb_mult
+            if cfg.vgg_mult > 0.0:
+                loss_dict["vgg_loss"] = self.vgg_loss(rgb, image) * cfg.vgg_mult
+        if self.training:
+            if "weights_list" in outputs:
+                loss_dict["interlevel_loss"] = cfg.interlevel_loss_mult * L.zipnerf_interlevel_loss(outputs["weights_list"],
+                                                                                                    outputs["ray_samples_list"])
+                assert metrics_dict is not None and "distortion" in metrics_dict
+                loss_dict["distortion_loss"] = cfg.distortion_loss_mult * metrics_dict["distortion"]
+                prop_depth_mult = cfg.prop_lidar_loss_mult * cfg.depth_mult
+                prop_carv_mult = cfg.prop_lidar_loss_mult * cfg.carving_mult
+                for i in range(len(cfg.sampling.num_proposal_samples)):
+                    loss_dict[f"depth_loss_{i}"] = prop_depth_mult * metrics_dict[f"depth_loss_{i}"]
+                    loss_dict[f"carving_loss_{i}"] = prop_carv_mult * metrics_dict[f"carving_loss_{i}"]
+            assert metrics_dict
+            for k, mult in (("depth_loss", cfg.depth_mult), ("intensity_loss", cfg.intensity_mult),
+                            ("carving_loss", cfg.carving_mult), ("ray_drop_loss", cfg.ray_drop_loss_mult)):
+                if k in metrics_dict:
+                    loss_dict[k] = mult * metrics_dict[k]
+            self.camera_optimizer.get_loss_dict(loss_dict)
+        return loss_dict
 
     @torch.no_grad()
     def get_image_metrics_and_images(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor]) -> Tuple[Dict[str, float], Dict[str, Tensor]]:

@@ -57,6 +57,28 @@ def step(model, rb, targets):
     return out, loss
 
 
+def neurad_batch(cfg, rb, n_cam, patch, device):
+    """The supervision of a NeuRAD training batch for get_metrics_dict / get_loss_dict: camera images at the decoder's
+    upsampled resolution, the lidar rows' distances and points (intensity in column 3), is_lidar / did_return over all
+    rays."""
+    gen = torch.Generator().manual_seed(6)
+    md = rb.metadata
+    up = cfg.rgb_upsample_factor
+    n_lidar = len(rb) - n_cam
+    return {"image": torch.rand(n_cam // (patch[0] * patch[1]), patch[0] * up, patch[1] * up, 3, generator=gen).to(device),
+            "is_lidar": md["is_lidar"], "did_return": md["did_return"], "distance": md["directions_norm"][n_cam:],
+            "lidar": torch.cat([50 * (torch.rand(n_lidar, 3, generator=gen) - 0.5), torch.rand(n_lidar, 1, generator=gen)],
+                               dim=1).to(device)}
+
+
+def neurad_step(model, rb, batch, patch):
+    """One step on NeuRAD's own objective (neurad.py:461-561): get_outputs (camera optimizer, module walk, lidar head, the
+    rgb decoder's torch training path) -> get_metrics_dict -> get_loss_dict, summed."""
+    out = model.get_outputs(rb, patch)
+    metrics = model.get_metrics_dict(out, batch)
+    return out, sum(model.get_loss_dict(out, batch, metrics).values())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--cam-rays", type=int, default=40960)
@@ -67,6 +89,9 @@ def main():
     ap.add_argument("--small-tables", action="store_true", help="2^14 / 2^13 slot tables instead of NeuRAD's 2^22 / 2^20")
     ap.add_argument("--camopt", choices=("off", "so3xr3", "scaled"), default="off")
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--objective", choices=("synthetic", "neurad"), default="synthetic",
+                    help="synthetic: feature / depth targets plus the regularisers; neurad: the mirror's get_metrics_dict / "
+                         "get_loss_dict on 32 x 32 camera patches, with a fixed stand-in perceptual loss")
     ap.add_argument("--preset", choices=nsb.PRESETS, default=None,
                     help="the model config and camera optimizer of a reference preset (overrides --camopt and the table sizes)")
     a = ap.parse_args()
@@ -95,13 +120,22 @@ def main():
     with torch.no_grad():
         ref = model.get_nff_outputs(rb, fused=True)
     targets = {"features": ref["features"] + 0.1, "depth": ref["depth"] * 1.1}
+    if a.objective == "neurad":
+        patch = (32, 32)
+        if a.cam_rays % (patch[0] * patch[1]):
+            raise SystemExit("--objective neurad needs --cam-rays in whole 32 x 32 patches")
+        batch = neurad_batch(cfg, rb, a.cam_rays, patch, dev)
+        model.vgg_loss = lambda rgb, image: (rgb - image).abs().mean()  # fixed stand-in: no VGG19 weights ship
+        step_fn = lambda model, rb, targets: neurad_step(model, rb, batch, patch)  # noqa: E731
+    else:
+        step_fn = step
     ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
     times = {"forward_and_losses": [], "backward": []}
     for it in range(a.warmup + a.steps):
         model.zero_grad(set_to_none=True)
         e0, e1, e2 = ev(), ev(), ev()
         e0.record()
-        out, loss = step(model, rb, targets)
+        out, loss = step_fn(model, rb, targets)
         e1.record()
         loss.backward()
         e2.record()
@@ -116,17 +150,22 @@ def main():
 
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             model.zero_grad(set_to_none=True)
-            step(model, rb, targets)[1].backward()
+            step_fn(model, rb, targets)[1].backward()
             torch.cuda.synchronize()
         for e in prof.key_averages():
             if "mean_bwd" in e.key or "isotropic_gaussian" in e.key or "neurad_encoding_bwd" in e.key:
                 kernels[e.key[:80]] = {"calls": e.count, "device_ms": getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0)) / 1e3}
     med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
     total = med["forward_and_losses"] + med["backward"]
-    res = {"what": "NFF training step (module walk + hand-written backward operators), device time", "rays": n,
+    what = "NFF training step (module walk + hand-written backward operators), device time"
+    if a.objective == "neurad":
+        what = "NFF training step on NeuRAD's objective (get_outputs -> get_metrics_dict -> get_loss_dict), device time"
+    res = {"what": what, "rays": n,
            "cam_rays": a.cam_rays, "lidar_rays": a.lidar_rays, "actors": a.actors, "tables": a.preset or ("small" if a.small_tables else "neurad-default"),
            "ms": med, "ms_total": total, "rays_per_s": n / total * 1e3, "loss": float(loss.detach()), "camopt": a.camopt,
            "gpu": torch.cuda.get_device_name(), "kernels": kernels}
+    if a.objective == "neurad":
+        res["objective"] = "neurad"
     print(json.dumps(res))
 
 
