@@ -141,6 +141,20 @@ int b200nerf_set_actors(b200nerf_ctx* ctx, int n_actors, int n_times, const floa
                         const float* rotations_6d, const float* positions, const uint8_t* present,
                         const float* sizes, const float* padding_host);
 
+/* DynamicActors.actor_editing (model_components/dynamic_actors.py:53-59, 181-249): render the actors at edited poses.
+ * An edited actor's box pose at a ray's time becomes t' = R (lateral, longitudinal, height) + t, then R' = Rz(rotation) R,
+ * where [R | t] is the interpolated box->world pose; everything downstream (ray-line cull, in-box tests, box-frame
+ * positions and directions, all three fields) uses the edited pose.  Semantics are the reference's:
+ *   - longitudinal, lateral and rotation all 0 means no edit, whatever `height` is (so all zeros clears the edit);
+ *   - index -1 edits every actor, otherwise actor min(index, n_actors - 1) truncated toward zero, a negative value
+ *     wrapping like torch indexing; a value that truncates below -n_actors is rejected (B200NERF_ERR_INVALID);
+ *   - the shifts are rounded to fp32; cos / sin of `rotation` are taken in double and rounded to fp32.
+ * The edit applies to b200nerf_nff_render_fwd and b200nerf_neurad_encoding_fwd (eval mode; the caller clears it for
+ * training) and never to the backward operators.  It is host-side state read at launch: no copy, no synchronisation,
+ * stream-ordered like the other set_* calls.  A no-op without actors; b200nerf_set_actors clears it. */
+int b200nerf_set_actor_edit(b200nerf_ctx* ctx, double lateral, double longitudinal, double height, double rotation,
+                            double index);
+
 /* SamplingSettings + ProposalNetworkSampler / PDFSampler constants (neurad.py:101-117,
  * ray_samplers.py:255-376, 569-666).  `u1_host` / `u2_host` are PDFSampler's eval-mode quantiles
  * `linspace(0, 1-1/nb, nb) + 1/(2nb)` for nb = n_prop1+1 and nb = n_nerf+1 (computed by the caller with

@@ -125,6 +125,10 @@ class B200NeuRADModel(NeuRADModel):
             params["static_scale"] = self.scene_box.aabb.max()
             be.load_params(self._b200_cfg, params)  # both rounds -> proposal_fields[1], the reference's effective behaviour
             be._owner = token
+        # the reference model's own actor_editing, read at every render: ADPipeline._update_actor_fids and the viewer
+        # sliders write it; get_boxes2world applies it in eval mode only (dynamic_actors.py:261-265)
+        ed = self.dynamic_actors.actor_editing
+        be.set_actor_edit(**({} if self.training else {k: ed[k] for k in _api.ACTOR_EDIT_KEYS}))
         return be
 
     # ---------------------------------------------------------------------------------------------- hot path

@@ -24,6 +24,14 @@ _fwd = torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
 _bwd = torch.amp.custom_bwd(device_type="cuda")
 
 
+def _refuse_edited(ctx) -> None:
+    """The backward operators differentiate the unedited actor poses, so a forward that rendered an actor edit
+    (eval mode, DynamicActors.actor_editing) has no backward here: raise instead of returning the wrong gradients."""
+    if ctx.edited:
+        raise RuntimeError("backward through a forward with an active actor edit: the gradients would be those of the "
+                           "unedited actor poses; clear dynamic_actors.actor_editing (or train in training mode)")
+
+
 class EncodingFn(Function):
     """NeuRADHashEncoding.forward: (features [N*S,D], directions [N,S,3]); gradients go to the hash tables, the sample
     means (when they require grad: camera optimisation) and -- for a field built with require_actor_grad (the main
@@ -34,7 +42,7 @@ class EncodingFn(Function):
     @_fwd
     def forward(ctx, be, field: int, mean, std, times, directions, flip, rotations_6d, positions, static_table, *actor_tables):
         out = be.neurad_encoding(field, mean, std, times, directions, flip=flip)
-        ctx.be, ctx.field = be, field
+        ctx.be, ctx.field, ctx.edited = be, field, be.actor_edit_active
         ctx.table_shapes = [static_table.shape] + [t.shape for t in actor_tables]
         ctx.save_for_backward(mean, std, times, flip, rotations_6d, positions)
         dirs = out.get("directions")
@@ -46,6 +54,7 @@ class EncodingFn(Function):
     @staticmethod
     @_bwd
     def backward(ctx, dfeatures, _ddirs):
+        _refuse_edited(ctx)
         mean, std, times, flip, rot6, pos = ctx.saved_tensors
         needs = ctx.needs_input_grad[9:]
         shapes, dev = ctx.table_shapes, dfeatures.device
@@ -75,7 +84,7 @@ class DensityFn(Function):
         # re-gathering 48 table entries per sample in the backward kernel
         want_feats = bool(ctx.needs_input_grad[7])
         out = be.neurad_encoding(field, mean, std, times, None, want_features=want_feats, want_density=True, flip=flip)
-        ctx.be, ctx.field = be, field
+        ctx.be, ctx.field, ctx.edited = be, field, be.actor_edit_active
         ctx.save_for_backward(mean, std, times, flip, out["density"], out.get("features"))
         ctx.decoder_shape = decoder_weight.shape
         ctx.table_shapes = [static_table.shape] + [t.shape for t in actor_tables]
@@ -84,6 +93,7 @@ class DensityFn(Function):
     @staticmethod
     @_bwd
     def backward(ctx, ddensity):
+        _refuse_edited(ctx)
         mean, std, times, flip, density, feats = ctx.saved_tensors
         needs = ctx.needs_input_grad[6:]
         shapes, dev = ctx.table_shapes, ddensity.device

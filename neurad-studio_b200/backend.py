@@ -24,6 +24,10 @@ def pdf_quantiles(num_samples: int) -> torch.Tensor:
     return u + 1.0 / (2 * num_bins)
 
 
+NO_ACTOR_EDIT = (0.0, 0.0, 0.0, 0.0, -1.0)  # (lateral, longitudinal, height, rotation, index): DynamicActors' defaults
+_lib_INVALID = -1  # B200NERF_ERR_INVALID
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
@@ -61,6 +65,10 @@ class B200Backend:
         # model in the process, so a model must re-bind whenever ANOTHER model (or a direct load_params call) came in between.
         self._owner = None
         self._dec_owner = None
+
+    # the actor edit the context holds (b200nerf_set_actors clears it), and whether it changes any actor's pose
+    _actor_edit = NO_ACTOR_EDIT
+    actor_edit_active = False
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
@@ -206,6 +214,7 @@ class B200Backend:
             )
         else:
             self._check(self.lib.b200nerf_set_actors(self._h, 0, 0, None, None, None, None, None, None))
+        self._actor_edit, self.actor_edit_active = NO_ACTOR_EDIT, False
         sp = cfg.sampling
         u1, u2 = pdf_quantiles(sp.num_proposal_samples[1]), pdf_quantiles(sp.num_nerf_samples)
         cu1 = (ctypes.c_float * u1.numel())(*u1.tolist())
@@ -218,6 +227,24 @@ class B200Backend:
                 float(cfg.rgb_upsample_factor**2),
             )
         )
+
+    def set_actor_edit(self, lateral: float = 0.0, longitudinal: float = 0.0, height: float = 0.0, rotation: float = 0.0,
+                       index: float = -1.0) -> None:
+        """DynamicActors.actor_editing (dynamic_actors.py:53-59, 181-249) for the following renders and module-level
+        encoding forwards, with the reference's semantics (include/b200nerf.h: b200nerf_set_actor_edit).  All zeros clears
+        it; load_params clears it too.  Only a change reaches the library.  Raises ValueError for an index that selects no
+        actor (below -n_actors), as the reference's indexing does."""
+        edit = tuple(float(v) for v in (lateral, longitudinal, height, rotation, index))
+        if edit == self._actor_edit:
+            return
+        rc = self.lib.b200nerf_set_actor_edit(self._h, *edit)
+        if rc == _lib_INVALID:  # the library has cleared the edit
+            self._actor_edit, self.actor_edit_active = NO_ACTOR_EDIT, False
+            raise ValueError(f"actor edit: {self.lib.b200nerf_last_error().decode()}")
+        self._check(rc)
+        self._actor_edit = edit
+        n_act = self.cfg.n_actors if self.cfg is not None else 0
+        self.actor_edit_active = n_act > 0 and any(v != 0.0 for v in (edit[0], edit[1], edit[3]))
 
     # ------------------------------------------------------------------------------------------ fused path
     def render(self, rays: Dict[str, torch.Tensor], want_trace: bool = False, want_intensity: bool = False,

@@ -226,8 +226,9 @@ __device__ __forceinline__ bool lane_patch_ray(const RenderParams& P, int64_t pa
 #endif
 // LAYOUT 0: the reference's torch-mode grids; 1: tiny-cuda-nn layout (tcnn-trained checkpoints, SURVEY 8f f3).  ACTORS /
 // TRACED = false leave the actor path / the trace stores out of the code: the untraced instances fit 64 registers without
-// spilling (sample_lane_kernel picks the instance).
-template <int LAYOUT, bool ACTORS, bool TRACED>
+// spilling (sample_lane_kernel picks the instance).  EDIT = true builds the actor frames with the actor edit
+// (lane_actor_candidates); only renders with an active edit launch those instances.
+template <int LAYOUT, bool ACTORS, bool TRACED, bool EDIT>
 __global__ void __launch_bounds__(kLaneThreads, NFF_SAMPLE_CTAS) nff_sample_lane_kernel(const __grid_constant__ RenderParams P,
                                                                                         float* __restrict__ scratch,
                                                                                         float* __restrict__ handoff) {
@@ -258,7 +259,7 @@ __global__ void __launch_bounds__(kLaneThreads, NFF_SAMPLE_CTAS) nff_sample_lane
     }
     int64_t ray;
     const bool active = lane_patch_ray(P, patch, lane_, &ray);
-    const LaneRay R = lane_ray_setup<ACTORS>(P, sc, tid, ray);
+    const LaneRay R = lane_ray_setup<ACTORS, EDIT>(P, sc, tid, ray);
     // inactive lanes write their (discarded) edges into the slab column instead of another ray's hand-over column
     float* col = active ? handoff + ray : sc.bins2 + tid;
     sample_ray_lane<LAYOUT, ACTORS, TRACED>(P, sc, R, tid, ray, active, col, active ? P.n_rays : (int64_t)kLaneThreads,
@@ -266,15 +267,16 @@ __global__ void __launch_bounds__(kLaneThreads, NFF_SAMPLE_CTAS) nff_sample_lane
   }
 }
 // the instance of a launch: `actors` = the scene has actors, `traced` = a proposal-stage trace is recorded (traced renders
-// take the instance with the actor path compiled in)
+// take the instance with the actor path compiled in), `edit` = an actor edit is active (the scene has actors)
 template <int LAYOUT>
-static auto sample_lane_kernel(bool actors, bool traced) {
-  return traced ? nff_sample_lane_kernel<LAYOUT, true, true>
-         : actors ? nff_sample_lane_kernel<LAYOUT, true, false>
-                  : nff_sample_lane_kernel<LAYOUT, false, false>;
+static auto sample_lane_kernel(bool actors, bool traced, bool edit) {
+  if (edit) return traced ? nff_sample_lane_kernel<LAYOUT, true, true, true> : nff_sample_lane_kernel<LAYOUT, true, false, true>;
+  return traced ? nff_sample_lane_kernel<LAYOUT, true, true, false>
+         : actors ? nff_sample_lane_kernel<LAYOUT, true, false, false>
+                  : nff_sample_lane_kernel<LAYOUT, false, false, false>;
 }
 
-template <int LAYOUT>
+template <int LAYOUT, bool EDIT>
 __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_kernel(const __grid_constant__ RenderParams P,
                                                                                       float* __restrict__ scratch,
                                                                                       const float* __restrict__ handoff) {
@@ -310,12 +312,13 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
     }
     int64_t ray;
     const bool active = lane_patch_ray(P, patch, tid & 31, &ray);
-    const LaneRay R = lane_ray_setup(P, sc, tid, ray);
+    const LaneRay R = lane_ray_setup<true, EDIT>(P, sc, tid, ray);
     shade_ray_lane<MlpLaneTc, LAYOUT>(P, sc, R, mlp, tid, ray, active, handoff + ray, P.n_rays);
   }
 }
 
 // Ray-per-lane variant (nff_lane.h), single fused kernel: a warp = 32 adjacent rays at the same sample index.
+template <bool EDIT>
 __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_kernel(const __grid_constant__ RenderParams P,
                                                                           float* __restrict__ scratch) {
   extern __shared__ __align__(128) unsigned char smem_lane[];
@@ -332,7 +335,7 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_
   for (int64_t unit = blockIdx.x; unit < lane_units(P); unit += gridDim.x) {
     int64_t ray;
     const bool active = lane_unit_ray(P, unit, tid, &ray);
-    render_ray_lane(P, sc, mlp, tid, ray, active);
+    render_ray_lane<MlpLaneTc, 0, EDIT>(P, sc, mlp, tid, ray, active);
   }
 }
 
@@ -1059,18 +1062,17 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
                                 (int)(tc_smem_bytes(kRenderWarps * 32) + kRenderWarps * sizeof(WarpSharedTc))));
   CUDA_TRY(cudaMalloc((void**)&c->d_status, sizeof(int)));
   CUDA_TRY(cudaMemset(c->d_status, 0, sizeof(int)));
-  CUDA_TRY(cudaFuncSetAttribute(nff_render_lane_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)lane_tc_smem_bytes()));
+  for (auto k : {nff_render_lane_kernel<false>, nff_render_lane_kernel<true>})
+    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lane_tc_smem_bytes()));
   c->lane_ctas = c->sm_count * (kLaneCtasPerSm > NFF_SAMPLE_CTAS ? kLaneCtasPerSm : NFF_SAMPLE_CTAS);
   CUDA_TRY(cudaMalloc((void**)&c->d_lane_scratch, sizeof(float) * lane_scratch_floats_per_cta() * c->lane_ctas));
-  CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)lane_tc_smem_bytes()));
-  CUDA_TRY(cudaFuncSetAttribute(nff_shade_lane_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)lane_tc_smem_bytes()));
+  for (auto k : {nff_shade_lane_kernel<0, false>, nff_shade_lane_kernel<1, false>, nff_shade_lane_kernel<0, true>,
+                 nff_shade_lane_kernel<1, true>})
+    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lane_tc_smem_bytes()));
   // (almost) all L1: the smallest carve-out that holds the 516 B edge table of each resident CTA
-  for (int i = 0; i < 4; ++i) {
-    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<0>(i & 1, i & 2), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
-    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<1>(i & 1, i & 2), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+  for (int i = 0; i < 8; ++i) {
+    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<0>(i & 1, i & 2, i & 4), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
+    CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<1>(i & 1, i & 2, i & 4), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
   }
   CUDA_TRY(cudaMalloc((void**)&c->d_minmax, 2 * sizeof(unsigned)));
   c->handoff_rays = (int64_t)1 << 21;
@@ -1337,6 +1339,13 @@ int b200nerf_set_actors(b200nerf_ctx* c, int n_actors, int n_times, const float*
   return 0;
 }
 
+int b200nerf_set_actor_edit(b200nerf_ctx* c, double lateral, double longitudinal, double height, double rotation, double index) {
+  REQUIRE(c, "ctx is NULL");
+  if (!resolve_actor_edit(c->actors, lateral, longitudinal, height, rotation, index))
+    return fail(B200NERF_ERR_INVALID, "actor edit index is below -n_actors");
+  return 0;
+}
+
 int b200nerf_set_sampling(b200nerf_ctx* c, int n_prop0, int n_prop1, int n_nerf, float lam, float scaling, float sky,
                           float hist_pad, const float* u1_host, const float* u2_host, const int* field_of_round,
                           float camera_area_scale) {
@@ -1431,6 +1440,7 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
   int64_t max_blocks = (int64_t)c->sm_count * (16 / WARPS);  // persistent: resident CTAs only, grid-stride over rays
   int blocks = (int)(blocks_needed < max_blocks ? blocks_needed : max_blocks);
   cudaStream_t st = (cudaStream_t)stream;
+  const bool edit = c->actors.edit_last > c->actors.edit_first;  // selects the edited lane-kernel instances
   if (c->mlp_mode == 3) {
     // sampling kernel -> [33][rays] spacing edges -> shading kernel; bundles larger than the hand-over buffer are
     // rendered in slices (whole 16-row tile bands when an image_width hint is given)
@@ -1462,11 +1472,13 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       const int64_t grid_a = patches < max_a ? patches : max_a, grid_b = groups < max_b ? groups : max_b;
       const bool actors = c->actors.n_actors > 0;
       if (c->layout == 1) {
-        sample_lane_kernel<1>(actors, traced)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
-        nff_shade_lane_kernel<1><<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        sample_lane_kernel<1>(actors, traced, edit)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        (edit ? nff_shade_lane_kernel<1, true> : nff_shade_lane_kernel<1, false>)<<<(int)grid_b, kLaneThreads, smem, st>>>(
+            Q, c->d_lane_scratch, c->d_handoff);
       } else {
-        sample_lane_kernel<0>(actors, traced)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
-        nff_shade_lane_kernel<0><<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        sample_lane_kernel<0>(actors, traced, edit)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
+        (edit ? nff_shade_lane_kernel<0, true> : nff_shade_lane_kernel<0, false>)<<<(int)grid_b, kLaneThreads, smem, st>>>(
+            Q, c->d_lane_scratch, c->d_handoff);
       }
     }
   } else if (c->mlp_mode == 2) {
@@ -1477,7 +1489,8 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       need = ((W + 31) / 32) * ((H + kLaneThreads / 32 - 1) / (kLaneThreads / 32));
     }
     int lane_blocks = (int)(need < c->lane_ctas ? need : c->lane_ctas);
-    nff_render_lane_kernel<<<lane_blocks, kLaneThreads, smem, st>>>(P, c->d_lane_scratch);
+    (edit ? nff_render_lane_kernel<true> : nff_render_lane_kernel<false>)<<<lane_blocks, kLaneThreads, smem, st>>>(
+        P, c->d_lane_scratch);
   } else if (c->mlp_mode == 1) {
     const size_t smem = tc_smem_bytes(WARPS * 32) + WARPS * sizeof(WarpSharedTc);
     nff_render_tc_kernel<WARPS><<<blocks, WARPS * 32, smem, st>>>(P);

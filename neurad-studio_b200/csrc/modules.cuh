@@ -47,8 +47,8 @@ struct EncodingArgs {
 // samples at a time.  F = 4 (main field) / F = 1 (proposal fields), at most 8 levels: a sample's feature row stays in
 // registers (neurad_encode_point_t), and the warp's 32 rows -- one contiguous block of `features` -- go out through a
 // shared-memory tile with an odd pitch so that the global stores are coalesced (lane = row wrote 32 different lines per
-// store instruction).
-template <int F>
+// store instruction).  EDIT: the frames carry the actor edit (only launched while one is active).
+template <int F, bool EDIT>
 __global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_fwd_kernel(const FieldGrids fg, const Actors A,
                                                                               const EncodingArgs a) {
   constexpr int kRow = 8 * F, kPitch = kRow + 1;
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(kModWarps * 32) neurad_encoding_fwd_kernel(con
     int left, right;
     float frac;
     keyframe_bracket(A, a.times[ray], left, right, frac);
-    for (int k = ln; k < A.n_actors; k += 32) actor_frame(A, k, left, right, frac, frames[k]);
+    for (int k = ln; k < A.n_actors; k += 32) actor_frame<EDIT>(A, k, left, right, frac, frames[k]);
   }
   __syncwarp();
   const int D = fg.stat.L * fg.stat.F;
@@ -125,10 +125,11 @@ inline bool launch_neurad_encoding_fwd(const FieldGrids& fg, const Actors& A, co
     if (smem > kSmemOptIn) err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (err == cudaSuccess) kernel<<<grid, kModWarps * 32, smem, stream>>>(fg, A, a);
   };
+  const bool edit = A.edit_last > A.edit_first;
   if (encode_bwd_fast_ok(fg, A.n_actors, 4))
-    launch(neurad_encoding_fwd_kernel<4>, 4);
+    launch(edit ? neurad_encoding_fwd_kernel<4, true> : neurad_encoding_fwd_kernel<4, false>, 4);
   else if (encode_bwd_fast_ok(fg, A.n_actors, 1))
-    launch(neurad_encoding_fwd_kernel<1>, 1);
+    launch(edit ? neurad_encoding_fwd_kernel<1, true> : neurad_encoding_fwd_kernel<1, false>, 1);
   else
     return false;
   return true;

@@ -544,6 +544,25 @@ NFF_D void normalize3(float v[3]) {  // F.normalize: v / max(|v|, 1e-12)
   v[2] = fdiv(v[2], n);
 }
 
+// DynamicActors.edit_boxes2world (model_components/dynamic_actors.py:181-249, flatten=False) for actor `a`: b1, b2, b3
+// are the rows of its box->world rotation R, t its centre.  The shift goes first, in the box frame and with the unedited
+// R: t' = R (lateral, longitudinal, height) + t; then R' = Rz(yaw) R.  Unedited actors return unchanged.  Every frame
+// builder calls this, so the culls, the in-box tests and the box-frame positions and directions all see the edit.
+NFF_D void edit_box_pose(const Actors& A, int a, float b1[3], float b2[3], const float b3[3], float t[3]) {
+  if (a < A.edit_first || a >= A.edit_last) return;
+  const float* s = A.edit_shift;
+  t[0] = fadd(fadd(fadd(fmul(b1[0], s[0]), fmul(b1[1], s[1])), fmul(b1[2], s[2])), t[0]);
+  t[1] = fadd(fadd(fadd(fmul(b2[0], s[0]), fmul(b2[1], s[1])), fmul(b2[2], s[2])), t[1]);
+  t[2] = fadd(fadd(fadd(fmul(b3[0], s[0]), fmul(b3[1], s[1])), fmul(b3[2], s[2])), t[2]);
+  const float c = A.edit_cos, sn = A.edit_sin;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {  // rows of Rz R: (c b1 - s b2, s b1 + c b2, b3)
+    const float x = b1[j], y = b2[j];
+    b1[j] = fsub(fmul(c, x), fmul(sn, y));
+    b2[j] = fadd(fmul(sn, x), fmul(c, y));
+  }
+}
+
 // DynamicActors.get_boxes2world (model_components/dynamic_actors.py:251-268) = interpolate_trajectories_6d
 // (utils/poses.py:90-150) + rotation_6d_to_matrix (cameras/camera_utils.py:422-443) + pose inverse
 // (utils/poses.py:42-55), followed by the ray-line culling of NeuRADHashEncoding._get_actor_indices
@@ -589,6 +608,7 @@ NFF_D void actor_candidates(const Actors& A, float time, const float o[3], const
       normalize3(b2);
       float b3[3] = {fsub(fmul(b1[1], b2[2]), fmul(b1[2], b2[1])), fsub(fmul(b1[2], b2[0]), fmul(b1[0], b2[2])),
                      fsub(fmul(b1[0], b2[1]), fmul(b1[1], b2[0]))};
+      edit_box_pose(A, a, b1, b2, b3, p + 6);
       // boxes2world rotation has rows b1,b2,b3; world2box rotation is its transpose
       R[0] = b1[0]; R[1] = b2[0]; R[2] = b3[0];
       R[3] = b1[1]; R[4] = b2[1]; R[5] = b3[1];

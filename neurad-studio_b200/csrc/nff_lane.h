@@ -53,6 +53,9 @@ NFF_D LaneScratch lane_scratch_of(float* base, int cta) {
 // --------------------------------------------------------------------------------------------- actors, per lane
 // Same computation as actor_candidates() (nff_device.h) for ONE ray: loop over all actors, keep those whose bounding
 // sphere the ray line passes (neurad_encoding.py:225-240), store [R^T | -R^T t], bounds and id in the scratch column.
+// EDIT: an actor edit is active (Actors::edit_first/last).  The cull then needs the edited centre, so the rotation is
+// built before it; without an edit the cheap centre test rejects first and the edit code is not compiled in.
+template <bool EDIT = false>
 NFF_D int lane_actor_candidates(const Actors& A, float time, const float o[3], const float d[3], const LaneScratch& sc,
                                 int tid, int* overflow) {
   int n = 0;
@@ -78,16 +81,21 @@ NFF_D int lane_actor_candidates(const Actors& A, float time, const float o[3], c
       p[i] = fadd(l_, fmul(fsub(r_, l_), frac));
     }
     bool valid = (A.present[(size_t)left * A.n_actors + a] | A.present[(size_t)right * A.n_actors + a]) != 0;
-    // cheap reject first: distance from the (unnormalised-rotation independent) box centre to the ray line
-    float v[3] = {fsub(p[6], o[0]), fsub(p[7], o[1]), fsub(p[8], o[2])};
-    float cx = fsub(fmul(v[1], d[2]), fmul(v[2], d[1]));
-    float cy = fsub(fmul(v[2], d[0]), fmul(v[0], d[2]));
-    float cz = fsub(fmul(v[0], d[1]), fmul(v[1], d[0]));
-    float dist = fsqrt(fadd(fadd(fmul(cx, cx), fmul(cy, cy)), fmul(cz, cz)));
-    if (!(valid && dist < ldg(A.radii + a) * 1.001f)) continue;
-    if (n >= kLaneMaxCand) {
-      *overflow = 1;
-      continue;
+    // distance from the box centre to the ray line (independent of the rotation, so without an edit it rejects first)
+    auto near_ray = [&]() {
+      float v[3] = {fsub(p[6], o[0]), fsub(p[7], o[1]), fsub(p[8], o[2])};
+      float cx = fsub(fmul(v[1], d[2]), fmul(v[2], d[1]));
+      float cy = fsub(fmul(v[2], d[0]), fmul(v[0], d[2]));
+      float cz = fsub(fmul(v[0], d[1]), fmul(v[1], d[0]));
+      float dist = fsqrt(fadd(fadd(fmul(cx, cx), fmul(cy, cy)), fmul(cz, cz)));
+      return valid && dist < ldg(A.radii + a) * 1.001f;
+    };
+    if (!EDIT) {
+      if (!near_ray()) continue;
+      if (n >= kLaneMaxCand) {
+        *overflow = 1;
+        continue;
+      }
     }
     float b1[3] = {p[0], p[1], p[2]};
     normalize3(b1);
@@ -96,6 +104,14 @@ NFF_D int lane_actor_candidates(const Actors& A, float time, const float o[3], c
     normalize3(b2);
     float b3[3] = {fsub(fmul(b1[1], b2[2]), fmul(b1[2], b2[1])), fsub(fmul(b1[2], b2[0]), fmul(b1[0], b2[2])),
                    fsub(fmul(b1[0], b2[1]), fmul(b1[1], b2[0]))};
+    if (EDIT) {
+      edit_box_pose(A, a, b1, b2, b3, p + 6);
+      if (!near_ray()) continue;
+      if (n >= kLaneMaxCand) {
+        *overflow = 1;
+        continue;
+      }
+    }
     float R[9] = {b1[0], b2[0], b3[0], b1[1], b2[1], b3[1], b1[2], b2[2], b3[2]};
     float* c = sc.cand + (size_t)n * kCandFloats * kLaneThreads + tid;
 #pragma unroll
@@ -537,7 +553,7 @@ NFF_D float lane_round0_edge(const Sampling& sp, int i) {
   lane_spacing_bounds(sp, kDefaultNear, kDefaultFar, &s_near, &s_far);
   return to_euclid(linspace01(i, kS0), s_near, s_far, sp);
 }
-template <bool ACTORS = true>
+template <bool ACTORS = true, bool EDIT = false>
 NFF_D LaneRay lane_ray_setup(const RenderParams& P, const LaneScratch& sc, int tid, int64_t ray) {
   const Sampling& sp = P.samp;
   LaneRay R;
@@ -553,7 +569,7 @@ NFF_D LaneRay lane_ray_setup(const RenderParams& P, const LaneScratch& sc, int t
   const float near_ = P.rays.nears ? ldg(P.rays.nears + ray) : kDefaultNear;
   lane_spacing_bounds(sp, near_, far_, &R.s_near, &R.s_far);
   int overflow = 0;
-  R.n_cand = ACTORS ? lane_actor_candidates(P.actors, R.time, R.o, R.d, sc, tid, &overflow) : 0;
+  R.n_cand = ACTORS ? lane_actor_candidates<EDIT>(P.actors, R.time, R.o, R.d, sc, tid, &overflow) : 0;
 #if defined(__CUDACC__)
   if (overflow && P.status) atomicExch(P.status, 3);
 #endif
@@ -761,9 +777,9 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
 
 // NeuRADModel.get_nff_outputs (models/neurad.py:368-421), eval mode, for the ray owned by this lane: both stages back to
 // back with the resampled edges handed over through the CTA's scratch slab.
-template <class Mlp, int LAYOUT = 0>
+template <class Mlp, int LAYOUT = 0, bool EDIT = false>
 NFF_D void render_ray_lane(const RenderParams& P, const LaneScratch& sc, Mlp& mlp, int tid, int64_t ray, bool active) {
-  const LaneRay R = lane_ray_setup(P, sc, tid, ray);
+  const LaneRay R = lane_ray_setup<true, EDIT>(P, sc, tid, ray);
   sample_ray_lane<LAYOUT>(P, sc, R, tid, ray, active, sc.bins2 + tid, kLaneThreads);
   shade_ray_lane<Mlp, LAYOUT>(P, sc, R, mlp, tid, ray, active, sc.bins2 + tid, kLaneThreads);
 }

@@ -39,6 +39,9 @@ NFF_D void keyframe_bracket(const Actors& A, float time, int& left, int& right, 
 // Gram-Schmidt'ed 6-D rotation + position (utils/poses.py:90-150), rotation_6d_to_matrix
 // (cameras/camera_utils.py:422-443), pose inverse (utils/poses.py:42-55).  Same op sequence as actor_candidates()
 // of the fused kernel, without the ray-line cull (a conservative optimisation there; the in-box test decides).
+// EDIT: apply the actor edit (edit_box_pose).  The backward operators use EDIT = false: their gradients are those of
+// the unedited poses, the only ones the reference trains.
+template <bool EDIT = false>
 NFF_D void actor_frame(const Actors& A, int a, int left, int right, float frac, ActorFrame& f) {
   const float* kl = A.keyframes + ((size_t)left * A.n_actors + a) * 9;
   const float* kr = A.keyframes + ((size_t)right * A.n_actors + a) * 9;
@@ -55,6 +58,7 @@ NFF_D void actor_frame(const Actors& A, int a, int left, int right, float frac, 
   normalize3(b2);
   float b3[3] = {fsub(fmul(b1[1], b2[2]), fmul(b1[2], b2[1])), fsub(fmul(b1[2], b2[0]), fmul(b1[0], b2[2])),
                  fsub(fmul(b1[0], b2[1]), fmul(b1[1], b2[0]))};
+  if (EDIT) edit_box_pose(A, a, b1, b2, b3, p + 6);
   float R[9] = {b1[0], b2[0], b3[0], b1[1], b2[1], b3[1], b1[2], b2[2], b3[2]};
   for (int i = 0; i < 3; ++i) {
     f.w2b[4 * i + 0] = R[3 * i + 0];

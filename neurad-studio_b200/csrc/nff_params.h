@@ -1,6 +1,7 @@
 // nff_params.h -- plain-old-data parameter blocks handed to the kernels (by value, in the kernel parameter
 // space) plus compile-time limits.  Shared between the CUDA build and the test-only host emulation.
 #pragma once
+#include <math.h>
 #include <stdint.h>
 
 #include "../../include/b200nerf.h"
@@ -86,7 +87,43 @@ struct Actors {
   const uint8_t* present;  // [T,A]
   const float* bounds;     // [A,3] = size/2 + padding
   const float* radii;      // [A]   = |bounds|
+  // DynamicActors.actor_editing (model_components/dynamic_actors.py:181-249), eval mode: actors [edit_first, edit_last)
+  // render at the edited pose t' = R shift + t, R' = Rz(yaw) R (edit_box_pose, nff_device.h).  Empty range: no edit.
+  int32_t edit_first, edit_last;
+  float edit_shift[3];       // (lateral, longitudinal, height), box frame
+  float edit_cos, edit_sin;  // cos / sin of the yaw, taken in double and rounded once
 };
+
+// The edit fields of `A` from the reference's actor_editing dict, resolved on the host (A.n_actors must be set).
+// - longitudinal, lateral and rotation all 0: no edit, even with a height (the reference tests only those three);
+// - index -1: every actor; otherwise actor min(index, n_actors - 1), truncated toward zero like
+//   torch.tensor([...], dtype=torch.int), a negative value wrapping like torch indexing.
+// Returns false, leaving A unedited, for an index that truncates below -n_actors (an IndexError in the reference).
+// With no actors there is nothing to edit and any values are accepted.
+inline bool resolve_actor_edit(Actors& A, double lateral, double longitudinal, double height, double rotation, double index) {
+  A.edit_first = A.edit_last = 0;
+  A.edit_shift[0] = A.edit_shift[1] = A.edit_shift[2] = 0.f;
+  A.edit_cos = 1.f;
+  A.edit_sin = 0.f;
+  const int n = A.n_actors;
+  if (n <= 0 || (longitudinal == 0.0 && lateral == 0.0 && rotation == 0.0)) return true;
+  int first = 0, last = n;
+  if (index != -1.0) {
+    const double m = (double)(n - 1) < index ? (double)(n - 1) : index;  // Python's min(index, n - 1), NaN included
+    const double k = trunc(m);
+    if (!(k >= -(double)n)) return false;  // also rejects NaN
+    first = (int)k < 0 ? (int)k + n : (int)k;
+    last = first + 1;
+  }
+  A.edit_first = first;
+  A.edit_last = last;
+  A.edit_shift[0] = (float)lateral;
+  A.edit_shift[1] = (float)longitudinal;
+  A.edit_shift[2] = (float)height;
+  A.edit_cos = (float)cos(rotation);
+  A.edit_sin = (float)sin(rotation);
+  return true;
+}
 
 struct Sampling {
   float lam, scaling, sky_distance, hist_pad, cam_area_scale;

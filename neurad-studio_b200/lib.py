@@ -92,6 +92,7 @@ SIGNATURES = {
     "b200nerf_set_appearance_per_sensor": (c_int, [c_void_p, c_void_p, c_int, c_int]),
     "b200nerf_set_actors": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     POINTER(c_float)]),
+    "b200nerf_set_actor_edit": (c_int, [c_void_p, c_double, c_double, c_double, c_double, c_double]),
     "b200nerf_set_sampling": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_float, c_float,
                                       POINTER(c_float), POINTER(c_float), POINTER(c_int), c_float]),
     "b200nerf_nff_render_fwd": (c_int, [c_void_p, POINTER(Rays), c_int64, POINTER(Outputs), POINTER(Trace), c_void_p]),

@@ -1001,6 +1001,19 @@ def make_camera_optimizer(config: Optional[CameraOptimizerConfig], num_cameras: 
     return cls(config=config, num_cameras=num_cameras, device=device, non_trainable_camera_indices=non_trainable_camera_indices)
 
 
+ACTOR_EDIT_KEYS = ("lateral", "longitudinal", "height", "rotation", "index")
+
+
+class DynamicActors:
+    """The non-parameter state of model_components/dynamic_actors.py:43-104 that rendering reads: `actor_editing`, the dict
+    the viewer sliders and ADPipeline._update_actor_fids write, with the reference's keys and defaults.  In eval mode every
+    render renders the actors at the edited poses (B200Backend.set_actor_edit has the semantics); training ignores it.
+    The trajectories themselves are the model's `dynamic_actors.*` parameters."""
+
+    def __init__(self) -> None:
+        self.actor_editing = {"lateral": 0.0, "longitudinal": 0.0, "rotation": 0.0, "index": -1.0, "height": 0.0}
+
+
 class NeuRADModel(nn.Module):
     """models/neurad.py:165 with the reference's parameter names: `state_dict()` / `load_state_dict()` speak the reference's
     dotted keys (`field.hashgrid.static_grid.hash_table`, ...; a `_model.` prefix as in `checkpoint["pipeline"]` is accepted),
@@ -1074,6 +1087,7 @@ class NeuRADModel(nn.Module):
         # get_loss_dict's perceptual term (neurad.py:260, 537-538): any callable (rgb, image) -> loss, e.g. the reference's
         # VGGPerceptualLossPix2Pix.  The library ships no VGG19 weights, so it is None until the caller assigns one.
         self.vgg_loss = None
+        self.dynamic_actors = DynamicActors()
 
     # -- nn.Module state dict in the reference's key format --------------------------------------------------------
     @staticmethod
@@ -1150,6 +1164,9 @@ class NeuRADModel(nn.Module):
             params["static_scale"] = self.static_scale
             be.load_params(self.config, params)
             be._owner = token
+        # DynamicActors.get_boxes2world edits only when not self.training (dynamic_actors.py:261-265)
+        ed = self.dynamic_actors.actor_editing
+        be.set_actor_edit(**({} if self.training else {k: ed[k] for k in ACTOR_EDIT_KEYS}))
         return be
 
     # -- forward API --------------------------------------------------------------------------------------------
