@@ -652,6 +652,27 @@ int b200nerf_lidar_losses_bwd(b200nerf_ctx* ctx, int64_t n, int n_prop, const fl
 int b200nerf_quantile(b200nerf_ctx* ctx, const float* x, int64_t n, float q, int lower_median, float* out, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* ---- camera image metrics ------------------------------------------------------------------------------- */
+
+/* PSNR and SSIM of the camera half of NeuRADModel.get_image_metrics_and_images (models/neurad.py:265-266, 585-586): what
+ * torchmetrics' PeakSignalNoiseRatio(data_range=1.0) and structural_similarity_index_measure (11 x 11 Gaussian window,
+ * sigma 1.5, k1 = 0.01, k2 = 0.03) return for images a, b of batch x height x width x channels fp32 values.  The SSIM
+ * definition is stated from memory, unpinned against torchmetrics; it is written out in csrc/image_metrics.cuh.
+ *
+ * a_strides / b_strides (host) = element strides of {batch, row, column, channel}, all >= 0, so channels-last [H, W, C]
+ * tensors and [B, C, H, W] views are read in place.  data_range <= 0 derives it as max(max a - min a, max b - min b) on the
+ * device; it enters SSIM's c1, c2 only (PSNR's range is 1).
+ *
+ * out_device (device, fp64) holds (batch + 1) x 4 values: {mse, psnr, ssim, data_range} of the whole batch, then of each
+ * image.  SSIM is the mean over the (height - 10) x (width - 10) windows inside the image, all channels, then over the
+ * batch.  Sums are fp64 in an order fixed by the shapes (bit-reproducible); a NaN pixel gives NaN.  No host
+ * synchronisation and no allocation: the partials live in the context, so calls on one context must not overlap.
+ * height, width >= 11, 1 <= batch <= 256 and at most 2^18 tiles of 32 x 32 windows x channels per call, else
+ * B200NERF_ERR_INVALID. */
+int b200nerf_image_metrics(b200nerf_ctx* ctx, const float* a, const float* b, int batch, int height, int width,
+                           int channels, const int64_t* a_strides, const int64_t* b_strides, float data_range,
+                           double* out_device, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,5 +6,6 @@ this directory, whose on-disk name carries a hyphen).
 from .config import (HashGridSettings, NeuRADConfig, NeuRADHashEncodingConfig, PRESETS, SamplingSettings, preset,  # noqa: F401
                      small_config)
 from .metrics import chamfer_distance  # noqa: F401
+from .metrics import ssim as structural_similarity_index_measure  # noqa: F401
 
 __version__ = "0.1.0"

@@ -1014,6 +1014,32 @@ class B200Backend:
                                                        self._stream))
         return (out, min_p, min_g) if want_minima else out
 
+    # ------------------------------------------------------------------------------------------ camera image metrics
+    def image_metrics(self, a: torch.Tensor, b: torch.Tensor, data_range: Optional[float] = None) -> torch.Tensor:
+        """PSNR (data range 1) and SSIM (11 x 11 Gaussian window, sigma 1.5) of image batches a, b [B, C, H, W], the shape
+        the reference hands its metrics (neurad.py:581-586).  Any strides are read in place, so `moveaxis(img, -1, 0)[None]`
+        of a channels-last [H, W, C] render needs no copy.  `data_range` None derives SSIM's range from the two images on
+        the device, max(a.max() - a.min(), b.max() - b.min()), as torchmetrics does.
+
+        Returns a [B + 1, 4] float64 tensor on the device: {mse, psnr, ssim, data_range} of the whole batch in row 0,
+        then of each image.  Nothing synchronises the host.  The partial sums live in the context: calls on one backend
+        must be ordered on one stream."""
+        if a.dim() != 4 or a.shape != b.shape:
+            raise ValueError(f"image metrics need two [B, C, H, W] tensors of one shape, got {tuple(a.shape)} and {tuple(b.shape)}")
+
+        def view(t):
+            t = t.detach()
+            if t.device != self.device or t.dtype != torch.float32:
+                t = t.to(device=self.device, dtype=torch.float32)
+            return t, (ctypes.c_int64 * 4)(t.stride(0), t.stride(2), t.stride(3), t.stride(1))
+
+        (ta, sa), (tb, sb) = view(a), view(b)
+        n, ch, h, w = ta.shape
+        out = torch.empty(n + 1, 4, dtype=torch.float64, device=self.device)
+        self._check(self.lib.b200nerf_image_metrics(self._h, _ptr(ta), _ptr(tb), n, h, w, ch, sa, sb,
+                                                    0.0 if data_range is None else float(data_range), _ptr(out), self._stream))
+        return out
+
     # ------------------------------------------------------------------------------------------ lidar training losses
     def _lidar_loss_rows(self, pred, prop, distance, did_return, intensity, gt_intensity, logits):
         """Flatten the lidar-row inputs of the lidar losses to what the C ABI takes (no host synchronisation)."""

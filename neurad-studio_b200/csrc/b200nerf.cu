@@ -14,6 +14,7 @@
 #include "modules.cuh"
 #include "lidar_eval.cuh"
 #include "lidar_loss.cuh"
+#include "image_metrics.cuh"
 
 using namespace nff;
 
@@ -77,6 +78,9 @@ struct b200nerf_ctx {
   float* d_dec_small = nullptr;       // in conv w [32*in] b [32] | convT w [32*32*9] b [32] | out conv w [3*32] b [3]
   bool mlp_attr_set = false;            // mlp_tc_kernel's dynamic shared memory opt-in done on this device
   float** d_grad_actor_ptrs = nullptr;  // [kModMaxActors] per-actor gradient accumulators of the current encoding_bwd call
+  // b200nerf_image_metrics (image_metrics.cuh): block partials of the statistics pass and the SSIM tiles
+  float* d_im_minmax = nullptr;   // [kImMaxBlocks][4]
+  double* d_im_sums = nullptr;    // [kImMaxBlocks] squared errors | [kSsimMaxTiles] SSIM tile sums
 };
 
 namespace {
@@ -1078,6 +1082,8 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
   c->handoff_rays = (int64_t)1 << 21;
   CUDA_TRY(cudaMalloc((void**)&c->d_handoff, sizeof(float) * (kS2 + 1) * c->handoff_rays));
   CUDA_TRY(cudaMalloc((void**)&c->d_grad_actor_ptrs, sizeof(float*) * kModMaxActors));
+  CUDA_TRY(cudaMalloc((void**)&c->d_im_minmax, sizeof(float) * 4 * kImMaxBlocks));
+  CUDA_TRY(cudaMalloc((void**)&c->d_im_sums, sizeof(double) * (kImMaxBlocks + kSsimMaxTiles)));
   *out = c;
   return 0;
 }
@@ -1093,6 +1099,8 @@ int b200nerf_destroy(b200nerf_ctx* c) {
   cudaFree(c->d_main_mlp_nn);
   cudaFree(c->d_lane_scratch);
   cudaFree(c->d_grad_actor_ptrs);
+  cudaFree(c->d_im_minmax);
+  cudaFree(c->d_im_sums);
   cudaFree(c->d_handoff);
   cudaFree(c->d_minmax);
   cudaFree(c->d_lidar_mlp);
@@ -2596,6 +2604,40 @@ int b200nerf_quantile(b200nerf_ctx* c, const float* x, int64_t n, float q, int l
   CUDA_TRY(cudaMemsetAsync(ws, 0, kLossStateBytes, s));
   select_hist_kernel<<<loss_blocks(n), kLossThreads, 0, s>>>(x, (int)n, 0, st, hist);
   select_rest(x, (int)n, q, lower_median, st, hist, out, s);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---- camera image metrics (image_metrics.cuh)
+int b200nerf_image_metrics(b200nerf_ctx* c, const float* a, const float* b, int batch, int height, int width, int channels,
+                           const int64_t* a_strides, const int64_t* b_strides, float data_range, double* out_device,
+                           void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(a && b && a_strides && b_strides && out_device, "NULL argument");
+  REQUIRE(batch >= 1 && batch <= kImMaxBlocks, "image metrics take 1 to 256 images per call");
+  REQUIRE(height >= kSsimWin && width >= kSsimWin, "SSIM's 11 x 11 window needs images of at least 11 x 11 pixels");
+  REQUIRE(channels >= 1 && (int64_t)width * channels <= 0x7fffffff, "channels must be >= 1 and width * channels below 2^31");
+  REQUIRE((int64_t)channels * height <= 0x7fffffff, "channels * height must be below 2^31");
+  REQUIRE(!(data_range != data_range), "data_range is NaN");
+  for (int k = 0; k < 4; ++k) REQUIRE(a_strides[k] >= 0 && b_strides[k] >= 0, "negative strides are not supported");
+  const int tiles_x = (width - (kSsimWin - 1) + kSsimTile - 1) / kSsimTile;
+  const int tiles_y = (height - (kSsimWin - 1) + kSsimTile - 1) / kSsimTile;
+  const int64_t tiles_per_image = (int64_t)tiles_x * tiles_y * channels;
+  REQUIRE(tiles_per_image * batch <= kSsimMaxTiles, "image metrics: more than 2^18 tiles of 32 x 32 windows x channels in one call");
+  DeviceGuard g(c->device);
+  const cudaStream_t s = (cudaStream_t)stream;
+  const ImageView va{a, a_strides[0], a_strides[1], a_strides[2], a_strides[3]};
+  const ImageView vb{b, b_strides[0], b_strides[1], b_strides[2], b_strides[3]};
+  const StatsWalk w = stats_walk(va, vb, height, width, channels);
+  const int rows = w.n_r1 * w.n_r2;
+  const int per_image = rows < kImMaxBlocks / batch ? rows : kImMaxBlocks / batch;
+  double* se_part = c->d_im_sums;
+  double* ssim_part = c->d_im_sums + kImMaxBlocks;
+  image_stats_kernel<<<dim3(per_image, batch), kImThreads, 0, s>>>(va, vb, w, c->d_im_minmax, se_part);
+  const SsimArgs args{va, vb, height, width, channels, tiles_x, tiles_y, per_image * batch, data_range};
+  ssim_tile_kernel<<<(unsigned)(tiles_per_image * batch), kImThreads, 0, s>>>(args, c->d_im_minmax, ssim_part);
+  image_metrics_finalize_kernel<<<1, kImThreads, 0, s>>>(batch, height, width, channels, per_image, (int)tiles_per_image,
+                                                         data_range, c->d_im_minmax, se_part, ssim_part, out_device);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -181,6 +181,8 @@ SIGNATURES = {
                                           c_void_p, c_int64, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200nerf_quantile": (c_int, [c_void_p, c_void_p, c_int64, c_float, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b200nerf_image_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int64),
+                                       POINTER(c_int64), c_float, c_void_p, c_void_p]),
 }
 
 _LIB = None

@@ -1,9 +1,12 @@
-"""NeuRAD's lidar evaluation metrics (models/neurad.py:268-271, 589-621) and the training PSNR of get_metrics_dict.
+"""NeuRAD's evaluation metrics (models/neurad.py:265-271, 568-621) and the training PSNR of get_metrics_dict.
 
 `chamfer_distance` is the reference's `nerfstudio.utils.math.chamfer_distance` on the library's all-pairs kernel
 (csrc/lidar_eval.cuh): exact fp32 per-pair squared distances from direct differences and fp64 sums, without the dense
 distance matrices of the reference's chunked `torch.cdist`.  The other four metrics are torch one-liners, as in the
 reference.
+
+`ssim` is the reference's `self.ssim`, torchmetrics' `structural_similarity_index_measure`, on the library's tile kernel
+(csrc/image_metrics.cuh), where the definition is written out.
 """
 from __future__ import annotations
 
@@ -50,3 +53,23 @@ def rmse(pred: Tensor, gt: Tensor) -> Tensor:
 def psnr(preds: Tensor, target: Tensor) -> Tensor:
     """torchmetrics' PeakSignalNoiseRatio(data_range=1.0) on one batch (neurad.py:265, 465): 10 log10(1 / mse)."""
     return -torch.log(torch.sum((preds - target) ** 2) / target.numel()) * (10 / math.log(10.0))
+
+
+def ssim(preds: Tensor, target: Tensor, data_range: Optional[float] = None) -> Tensor:
+    """torchmetrics' structural_similarity_index_measure(preds, target) with its defaults, the reference's `self.ssim`
+    (neurad.py:266, 586), as a 0-d tensor of the input dtype on the input's CUDA device.
+
+    The definition is written from memory, unpinned against torchmetrics (the package is not a dependency, and the one
+    test that compares with it, in tests/test_zz_image_metrics_gpu.py, runs only where it is installed): an 11 x 11
+    Gaussian window of sigma 1.5, normalised in fp32 and applied per channel to preds, target, their squares and their
+    product; c1 = (0.01 R)^2 and c2 = (0.03 R)^2 with R = `data_range`, or max(preds.max() - preds.min(), target.max() -
+    target.min()) when it is None; variances clamped at 0; and the mean of
+    (2 mu_p mu_t + c1)(2 cov + c2) / ((mu_p^2 + mu_t^2 + c1)(var_p + var_t + c2)) over the (H - 10) x (W - 10) windows that
+    lie inside the image (what torchmetrics keeps after its reflect padding and crop), all channels, then over the batch.
+
+    preds / target are [B, C, H, W] with H, W >= 11; non-contiguous views are read in place.  Other window sizes,
+    non-Gaussian windows and multi-scale SSIM are not provided."""
+    from .nerfstudio_api import get_backend
+
+    with torch.no_grad():
+        return get_backend(preds.device).image_metrics(preds, target, data_range)[0, 2].to(preds.dtype)

@@ -1084,6 +1084,11 @@ class NeuRADModel(nn.Module):
         # lidar metrics (neurad.py:268-271); the chamfer distance runs on the library's all-pairs kernel
         self.median_l2, self.mean_rel_l2, self.rmse = M.median_l2, M.mean_rel_l2, M.rmse
         self.chamfer_distance = lambda pred, gt: M.chamfer_distance(pred, gt, 1_000, True)
+        # camera metrics (neurad.py:265-267).  PSNR and SSIM run on the library's kernels; LPIPS needs network weights the
+        # library does not ship, so `lpips` is any callable (image, rgb) -> value on [1, 3, H, W] tensors, e.g. torchmetrics'
+        # LearnedPerceptualImagePatchSimilarity(normalize=True), and camera batches are refused until the caller assigns one.
+        self.ssim = M.ssim
+        self.lpips = None
         # get_loss_dict's perceptual term (neurad.py:260, 537-538): any callable (rgb, image) -> loss, e.g. the reference's
         # VGGPerceptualLossPix2Pix.  The library ships no VGG19 weights, so it is None until the caller assigns one.
         self.vgg_loss = None
@@ -1518,19 +1523,38 @@ class NeuRADModel(nn.Module):
 
     @torch.no_grad()
     def get_image_metrics_and_images(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor]) -> Tuple[Dict[str, float], Dict[str, Tensor]]:
-        """The lidar half of neurad.py:563-621, on the outputs / batch of get_outputs_for_lidar: depth median L2, depth mean
-        relative L2, intensity RMSE, ray-drop accuracy and chamfer distance, with the reference's keys and values.  Like the
-        reference it fills batch["is_lidar"] / batch["did_return"] when they are absent, and the chamfer distance is a 0-d
-        tensor (the mean range of the measured returns) when there are no predicted or no measured returns, a float
-        otherwise.  images_dict stays empty.
+        """neurad.py:563-621 on the outputs / batch of an evaluation render.
 
-        A camera batch ("image") raises: PSNR / SSIM / LPIPS need torchmetrics and LPIPS weights, which this library does
-        not ship, and partial camera metrics are never returned."""
-        if "image" in batch:
-            raise NotImplementedError("camera metrics (PSNR / SSIM / LPIPS) need torchmetrics and LPIPS weights, which "
-                                      "neurad_studio_b200 does not ship; evaluate camera images with the reference's model")
+        Lidar batches ("lidar"): depth median L2, depth mean relative L2, intensity RMSE, ray-drop accuracy and chamfer
+        distance, with the reference's keys and values.  Like the reference it fills batch["is_lidar"] / batch["did_return"]
+        when they are absent, and the chamfer distance is a 0-d tensor (the mean range of the measured returns) when there
+        are no predicted or no measured returns, a float otherwise.
+
+        Camera batches ("image", [H, W, 3] next to outputs["rgb"]): psnr, ssim and lpips as floats and images_dict["img"],
+        the ground truth beside the render.  PSNR and SSIM come from one call of the library's kernels and one
+        device-to-host copy; LPIPS is whatever callable the caller assigned to `self.lpips`.  Without one a camera batch
+        raises before any work: LPIPS needs network weights the library does not ship, and a partial camera dict is never
+        returned.  A batch with both keys returns both halves.
+
+        Not provided: the colour-mapped entries of the reference's images_dict ("depth", and "accumulation" /
+        "prop_depth_i" under config.verbose), which need matplotlib's colour tables."""
+        if "image" in batch and self.lpips is None:
+            raise NotImplementedError("camera metrics (PSNR / SSIM / LPIPS): the reference takes them from torchmetrics and LPIPS "
+                                      "weights, which neurad_studio_b200 does not ship.  PSNR and SSIM run on the library's "
+                                      "kernels, but LPIPS needs a callable: assign model.lpips = fn(image, rgb) -> value for "
+                                      "[1, 3, H, W] tensors (e.g. torchmetrics' LearnedPerceptualImagePatchSimilarity"
+                                      "(normalize=True)) to evaluate camera images")
         metrics_dict: Dict[str, float] = {}
         images_dict: Dict[str, Tensor] = {}
+        if "image" in batch:
+            image, rgb = batch["image"].to(self.static_scale.device), outputs["rgb"]
+            images_dict["img"] = torch.cat([image, rgb], dim=1)
+            # [H, W, C] -> [1, C, H, W] views, as the reference hands them to its metrics (neurad.py:581-582)
+            image = torch.moveaxis(image, -1, 0)[None, ...]
+            rgb = torch.moveaxis(rgb, -1, 0)[None, ...]
+            # row 0 = {mse, psnr, ssim, data_range} of the batch: both floats in one device-to-host copy
+            _, metrics_dict["psnr"], metrics_dict["ssim"], _ = get_backend(rgb.device).image_metrics(image, rgb)[0].tolist()
+            metrics_dict["lpips"] = float(self.lpips(image, rgb))
         if "lidar" in batch:
             device = self.static_scale.device
             points = batch["lidar"].to(device)
