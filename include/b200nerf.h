@@ -589,6 +589,39 @@ int b200nerf_raygen_pinhole(b200nerf_ctx* ctx, const float* c2w_host, float fx, 
                             float time_to_center_pixel, float* origins, float* directions, float* pixel_area,
                             float* times, void* stream);
 
+/* One camera of a `Cameras` batch (cameras/cameras.py) with the AD dataparsers' rolling-shutter metadata. */
+enum {
+  B200NERF_CAMERA_PERSPECTIVE = 0, /* CameraType.PERSPECTIVE */
+  B200NERF_CAMERA_FISHEYE = 1      /* CameraType.FISHEYE: equidistant mapping (cameras.py:800-815), e.g. ZOD */
+};
+enum {
+  B200NERF_RS_VERTICAL = 0,           /* time offset from the row: top to bottom (PandaSet, nuScenes, ...) */
+  B200NERF_RS_HORIZONTAL = 1,         /* metadata["rs_direction"] == "Horizontal": from the column (Waymo) */
+  B200NERF_RS_HORIZONTAL_REVERSED = 2 /* "Horizontal_reversed": the negated column offset, time_to_center_pixel included */
+};
+typedef struct b200nerf_camera {
+  float c2w[12]; /* 3x4 row major, OpenGL convention */
+  float fx, fy, cx, cy;
+  int width, height;
+  int camera_type;      /* B200NERF_CAMERA_* */
+  float distortion[6];  /* k1, k2, k3, k4, p1, p2 (camera_utils.py:655-758); all zero = no undistortion */
+  float time;
+  float velocity[3];    /* read only when has_velocity != 0 */
+  int has_velocity;     /* 0: no rolling shutter, every ray at `time` from the camera centre */
+  float rolling_shutter_time, time_to_center_pixel;
+  int rs_direction;     /* B200NERF_RS_* */
+} b200nerf_camera;
+
+/* Cameras.generate_rays for one PERSPECTIVE or FISHEYE camera with radial / tangential distortion and a vertical or
+ * horizontal rolling shutter, over the same strided pixel grid and with the same outputs as b200nerf_raygen_pinhole
+ * (which is this call with a perspective, undistorted, vertical descriptor).  Undistortion is the reference's 10
+ * Newton steps on the normalised coordinates of each pixel and of its +x / +y offsets; a fisheye camera whose principal
+ * point lies on a pixel centre gives that pixel a NaN direction, as the reference does.  Another camera_type returns
+ * B200NERF_ERR_UNSUPPORTED, another rs_direction B200NERF_ERR_INVALID. */
+int b200nerf_raygen_camera(b200nerf_ctx* ctx, const b200nerf_camera* camera, int row0, int row_step, int n_rows,
+                           int col0, int col_step, int n_cols, float* origins, float* directions, float* pixel_area,
+                           float* times, void* stream);
+
 /* Lidars._generate_rays_from_points, assume_ego_compensated=True (cameras/lidars.py:399-460): points [P,
  * point_stride] = (x,y,z,intensity,dt,...) in the lidar frame -> rays; `distance` (optional) = the range. */
 int b200nerf_raygen_lidar_points(b200nerf_ctx* ctx, const float* l2w_host, const float* points, int point_stride,

@@ -32,6 +32,44 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
+def is_pinhole_camera(cam) -> bool:
+    """True for an undistorted PERSPECTIVE camera with a top-to-bottom shutter: the model of `raygen_pinhole`."""
+    dist = getattr(cam, "distortion_params", None)
+    return (getattr(cam, "camera_type", "perspective") == "perspective" and getattr(cam, "rs_direction", "Vertical") == "Vertical"
+            and (dist is None or not bool((torch.as_tensor(dist) != 0).any())))
+
+
+def camera_descriptor(cam) -> "_lib.Camera":
+    """b200nerf_camera of a scene.PinholeCamera; ValueError for an unknown camera_type or rs_direction, or a distortion
+    vector that does not have 6 entries (k1, k2, k3, k4, p1, p2)."""
+    # a camera object without the model fields (written before they existed) is the undistorted perspective default
+    camera_type = getattr(cam, "camera_type", "perspective")
+    rs_direction = getattr(cam, "rs_direction", "Vertical")
+    distortion = getattr(cam, "distortion_params", None)
+    if camera_type not in _lib.CAMERA_TYPES:
+        raise ValueError(f"camera_type {camera_type!r}: expected one of {sorted(_lib.CAMERA_TYPES)}")
+    if rs_direction not in _lib.RS_DIRECTIONS:
+        raise ValueError(f"rs_direction {rs_direction!r}: expected one of {sorted(_lib.RS_DIRECTIONS)}")
+    dist = [0.0] * 6
+    if distortion is not None:
+        dist = torch.as_tensor(distortion, dtype=torch.float32).reshape(-1).tolist()
+        if len(dist) != 6:
+            raise ValueError(f"distortion_params must hold 6 values (k1, k2, k3, k4, p1, p2), got {len(dist)}")
+    d = _lib.Camera()
+    d.c2w[:] = torch.as_tensor(cam.c2w, dtype=torch.float32).reshape(-1).tolist()
+    d.fx, d.fy, d.cx, d.cy = cam.fx, cam.fy, cam.cx, cam.cy
+    d.width, d.height = cam.width, cam.height
+    d.camera_type = _lib.CAMERA_TYPES[camera_type]
+    d.distortion[:] = dist
+    d.time = cam.time
+    if cam.velocity is not None:
+        d.velocity[:] = torch.as_tensor(cam.velocity, dtype=torch.float32).reshape(-1).tolist()
+        d.has_velocity = 1
+    d.rolling_shutter_time, d.time_to_center_pixel = cam.rolling_shutter_time, cam.time_to_center_pixel
+    d.rs_direction = _lib.RS_DIRECTIONS[rs_direction]
+    return d
+
+
 def grid_desc(g: HashGridSettings, scalings: Optional[torch.Tensor] = None) -> GridDesc:
     d = GridDesc()
     d.num_levels, d.features_per_level, d.log2_hashmap_size = g.num_levels, g.hashgrid_dim, g.log2_hashmap_size
@@ -930,24 +968,27 @@ class B200Backend:
                 raise ValueError("pre-allocated ray buffer has the wrong layout")
         return bufs
 
-    def raygen_pinhole(self, cam, row0: int = 0, row_step: int = 1, col0: int = 0, col_step: int = 1,
-                       out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
-        """Cameras.generate_rays for one pinhole camera (scene.PinholeCamera) over a strided pixel grid.
+    def raygen_camera(self, cam, row0: int = 0, row_step: int = 1, col0: int = 0, col_step: int = 1,
+                      out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+        """Cameras.generate_rays for one camera (scene.PinholeCamera: perspective or fisheye, optional k1..k4, p1, p2
+        distortion, vertical or horizontal rolling shutter) over a strided pixel grid.
         `out` may hold pre-allocated (slices of) origins/directions/pixel_area/times buffers."""
+        desc = camera_descriptor(cam)
         n_rows = len(range(row0, cam.height, row_step))
         n_cols = len(range(col0, cam.width, col_step))
         n = n_rows * n_cols
         o, d, a, t = self._ray_buffers(n, out)
-        c2w = (ctypes.c_float * 12)(*cam.c2w.reshape(-1).tolist())
-        vel = (ctypes.c_float * 3)(*cam.velocity.tolist()) if cam.velocity is not None else None
         self._check(
-            self.lib.b200nerf_raygen_pinhole(
-                self._h, c2w, cam.fx, cam.fy, cam.cx, cam.cy, cam.height, cam.width, row0, row_step, n_rows, col0,
-                col_step, n_cols, cam.time, vel, cam.rolling_shutter_time, cam.time_to_center_pixel, _ptr(o), _ptr(d),
-                _ptr(a), _ptr(t), self._stream,
-            )
+            self.lib.b200nerf_raygen_camera(self._h, ctypes.byref(desc), row0, row_step, n_rows, col0, col_step, n_cols,
+                                            _ptr(o), _ptr(d), _ptr(a), _ptr(t), self._stream)
         )
         return {"origins": o, "directions": d, "pixel_area": a, "times": t, "shape": (n_rows, n_cols)}
+
+    def raygen_pinhole(self, cam, row0: int = 0, row_step: int = 1, col0: int = 0, col_step: int = 1,
+                       out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+        """raygen_camera under its original name (a default scene.PinholeCamera is an undistorted perspective camera
+        with a top-to-bottom shutter)."""
+        return self.raygen_camera(cam, row0, row_step, col0, col_step, out)
 
     def raygen_lidar_points(self, scan, points: Optional[torch.Tensor] = None,
                             out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:

@@ -15,6 +15,7 @@
 #include "lidar_eval.cuh"
 #include "lidar_loss.cuh"
 #include "image_metrics.cuh"
+#include "camera_rays.h"
 
 using namespace nff;
 
@@ -882,60 +883,21 @@ __global__ void __launch_bounds__(128) mlp_tc_kernel(const MlpArgs a, const floa
   }
 }
 
-// Cameras._generate_rays_from_coords, pinhole + rolling shutter (cameras/cameras.py:633-667,793-798,898-969)
-struct PinholeArgs {
-  float c2w[12];
-  float fx, fy, cx, cy;
-  int height, width, row0, row_step, n_rows, col0, col_step, n_cols;
-  float time, vel[3], rs_time, ttc;
-  int has_vel;
-};
-__device__ __forceinline__ void cam_dir(const PinholeArgs& a, float u, float v, float out[3], float* norm) {
-  // direction (u, -v, -1) rotated by c2w: sum over columns of dir_j * R[i][j]  (cameras.py:902-904)
-  float dx = u, dy = -v, dz = -1.0f;
-  float r[3];
-#pragma unroll
-  for (int i = 0; i < 3; ++i)
-    r[i] = fadd(fadd(fmul(dx, a.c2w[4 * i + 0]), fmul(dy, a.c2w[4 * i + 1])), fmul(dz, a.c2w[4 * i + 2]));
-  float n = fsqrt(fadd(fadd(fmul(r[0], r[0]), fmul(r[1], r[1])), fmul(r[2], r[2])));
-  n = fmaxf(n, 8.8817841970012523e-16f);  // camera_utils.py:30 (_EPS = 4 * float64 eps, cast to fp32)
-  out[0] = fdiv(r[0], n); out[1] = fdiv(r[1], n); out[2] = fdiv(r[2], n);
-  *norm = n;
-}
-__global__ void raygen_pinhole_kernel(PinholeArgs a, float* __restrict__ origins, float* __restrict__ dirs,
-                                      float* __restrict__ area, float* __restrict__ times) {
+// Cameras._generate_rays_from_coords for PERSPECTIVE / FISHEYE cameras, with or without distortion (camera_rays.h).  The
+// undistorted perspective instance carries no Newton iteration and no sin / cos; the shutter direction is uniform.
+template <bool kFisheye, bool kDistorted>
+__global__ void raygen_camera_kernel(CameraArgs a, float* __restrict__ origins, float* __restrict__ dirs,
+                                     float* __restrict__ area, float* __restrict__ times) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)a.n_rows * a.n_cols) return;
-  int r = (int)(i / a.n_cols), c = (int)(i % a.n_cols);
-  float y = (float)(a.row0 + r * a.row_step) + 0.5f, x = (float)(a.col0 + c * a.col_step) + 0.5f;
-  float u0 = fdiv(fsub(x, a.cx), a.fx), v0 = fdiv(fsub(y, a.cy), a.fy);
-  float u1 = fdiv(fadd(fsub(x, a.cx), 1.0f), a.fx), v1 = fdiv(fadd(fsub(y, a.cy), 1.0f), a.fy);
-  float d0[3], dxo[3], dyo[3], n0, n1;
-  cam_dir(a, u0, v0, d0, &n0);
-  cam_dir(a, u1, v0, dxo, &n1);
-  cam_dir(a, u0, v1, dyo, &n1);
-  float ex[3], ey[3];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    ex[k] = fsub(d0[k], dxo[k]);
-    ey[k] = fsub(d0[k], dyo[k]);
-  }
-  float dx = fsqrt(fadd(fadd(fmul(ex[0], ex[0]), fmul(ex[1], ex[1])), fmul(ex[2], ex[2])));
-  float dy = fsqrt(fadd(fadd(fmul(ey[0], ey[0]), fmul(ey[1], ey[1])), fmul(ey[2], ey[2])));
-  float o[3] = {a.c2w[3], a.c2w[7], a.c2w[11]};
-  float t = a.time;
-  if (a.has_vel) {
-    float toff = fadd(fmul(fsub(fdiv(y, (float)a.height), 0.5f), a.rs_time), a.ttc);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) o[k] = fadd(o[k], fmul(a.vel[k], toff));
-    t = fadd(t, toff);
-  }
+  float o[3], d[3], pa, t;
+  camera_ray<kFisheye, kDistorted>(a, i, o, d, &pa, &t);
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     origins[3 * i + k] = o[k];
-    dirs[3 * i + k] = d0[k];
+    dirs[3 * i + k] = d[k];
   }
-  area[i] = fmul(dx, dy);
+  area[i] = pa;
   times[i] = t;
 }
 
@@ -2404,22 +2366,52 @@ int b200nerf_raygen_pinhole(b200nerf_ctx* c, const float* c2w_host, float fx, fl
                             int width, int row0, int row_step, int n_rows, int col0, int col_step, int n_cols,
                             float time, const float* velocity_host, float rs_time, float ttc, float* origins,
                             float* directions, float* pixel_area, float* times, void* stream) {
-  REQUIRE(c && c2w_host && origins && directions && pixel_area && times, "NULL argument");
+  REQUIRE(c2w_host, "NULL argument");
+  b200nerf_camera cam{};
+  memcpy(cam.c2w, c2w_host, sizeof(float) * 12);
+  cam.fx = fx; cam.fy = fy; cam.cx = cx; cam.cy = cy;
+  cam.width = width; cam.height = height;
+  cam.camera_type = B200NERF_CAMERA_PERSPECTIVE;
+  cam.time = time;
+  cam.has_velocity = velocity_host != nullptr;
+  if (velocity_host) memcpy(cam.velocity, velocity_host, sizeof(float) * 3);
+  cam.rolling_shutter_time = rs_time; cam.time_to_center_pixel = ttc;
+  cam.rs_direction = B200NERF_RS_VERTICAL;
+  return b200nerf_raygen_camera(c, &cam, row0, row_step, n_rows, col0, col_step, n_cols, origins, directions, pixel_area,
+                                times, stream);
+}
+
+int b200nerf_raygen_camera(b200nerf_ctx* c, const b200nerf_camera* cam, int row0, int row_step, int n_rows, int col0,
+                           int col_step, int n_cols, float* origins, float* directions, float* pixel_area, float* times,
+                           void* stream) {
+  REQUIRE(c && cam && origins && directions && pixel_area && times, "NULL argument");
   REQUIRE(n_rows >= 0 && n_cols >= 0 && row_step >= 1 && col_step >= 1, "bad pixel grid");
+  if (cam->camera_type != B200NERF_CAMERA_PERSPECTIVE && cam->camera_type != B200NERF_CAMERA_FISHEYE)
+    return fail(B200NERF_ERR_UNSUPPORTED, "camera_type must be PERSPECTIVE (0) or FISHEYE (1)");
+  REQUIRE(cam->rs_direction == B200NERF_RS_VERTICAL || cam->rs_direction == B200NERF_RS_HORIZONTAL ||
+              cam->rs_direction == B200NERF_RS_HORIZONTAL_REVERSED,
+          "rs_direction must be VERTICAL (0), HORIZONTAL (1) or HORIZONTAL_REVERSED (2)");
   if (n_rows == 0 || n_cols == 0) return 0;
   DeviceGuard g(c->device);
-  PinholeArgs a{};
-  memcpy(a.c2w, c2w_host, sizeof(float) * 12);
-  a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
-  a.height = height; a.width = width;
+  CameraArgs a{};
+  memcpy(a.c2w, cam->c2w, sizeof(float) * 12);
+  a.fx = cam->fx; a.fy = cam->fy; a.cx = cam->cx; a.cy = cam->cy;
+  memcpy(a.dist, cam->distortion, sizeof(float) * 6);
+  a.height = cam->height; a.width = cam->width;
   a.row0 = row0; a.row_step = row_step; a.n_rows = n_rows;
   a.col0 = col0; a.col_step = col_step; a.n_cols = n_cols;
-  a.time = time; a.rs_time = rs_time; a.ttc = ttc;
-  a.has_vel = velocity_host != nullptr;
-  if (velocity_host) memcpy(a.vel, velocity_host, sizeof(float) * 3);
+  a.time = cam->time; a.rs_time = cam->rolling_shutter_time; a.ttc = cam->time_to_center_pixel;
+  a.has_vel = cam->has_velocity != 0;
+  if (a.has_vel) memcpy(a.vel, cam->velocity, sizeof(float) * 3);
+  a.rs_dir = cam->rs_direction;
+  // all-zero parameters: the reference skips undistortion, and one Newton step would return x unchanged anyway
+  bool distorted = false;
+  for (int k = 0; k < 6; ++k) distorted |= a.dist[k] != 0.0f;
+  const bool fisheye = cam->camera_type == B200NERF_CAMERA_FISHEYE;
+  auto kernel = fisheye ? (distorted ? raygen_camera_kernel<true, true> : raygen_camera_kernel<true, false>)
+                        : (distorted ? raygen_camera_kernel<false, true> : raygen_camera_kernel<false, false>);
   int64_t n = (int64_t)n_rows * n_cols;
-  raygen_pinhole_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, origins, directions,
-                                                                                        pixel_area, times);
+  kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, origins, directions, pixel_area, times);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -78,6 +78,19 @@ class RgbDecoderParams(ctypes.Structure):
                 ("in_conv", ConvParams), ("block", (ConvBnParams * 2) * 4), ("up_conv", ConvParams), ("out_conv", ConvParams)]
 
 
+CAMERA_TYPES = {"perspective": 0, "fisheye": 1}  # b200nerf_camera.camera_type
+RS_DIRECTIONS = {"Vertical": 0, "Horizontal": 1, "Horizontal_reversed": 2}  # b200nerf_camera.rs_direction
+
+
+class Camera(ctypes.Structure):
+    """b200nerf_camera: one PERSPECTIVE / FISHEYE camera with distortion and rolling-shutter metadata."""
+
+    _fields_ = [("c2w", c_float * 12), ("fx", c_float), ("fy", c_float), ("cx", c_float), ("cy", c_float),
+                ("width", c_int32), ("height", c_int32), ("camera_type", c_int32), ("distortion", c_float * 6),
+                ("time", c_float), ("velocity", c_float * 3), ("has_velocity", c_int32),
+                ("rolling_shutter_time", c_float), ("time_to_center_pixel", c_float), ("rs_direction", c_int32)]
+
+
 SIGNATURES = {
     "b200nerf_last_error": (c_char_p, []),
     "b200nerf_version": (c_int, []),
@@ -165,6 +178,8 @@ SIGNATURES = {
     "b200nerf_raygen_pinhole": (c_int, [c_void_p, POINTER(c_float), c_float, c_float, c_float, c_float, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_int, c_int, c_float, POINTER(c_float), c_float,
                                         c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200nerf_raygen_camera": (c_int, [c_void_p, POINTER(Camera), c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p]),
     "b200nerf_raygen_lidar_grid": (c_int, [c_void_p, POINTER(c_float), c_float, c_float, c_int, c_int, c_double, c_float,
                                            c_float, POINTER(c_float), c_float, c_float, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p]),

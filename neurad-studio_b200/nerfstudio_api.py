@@ -40,7 +40,7 @@ from torch import Tensor, nn
 
 from . import autograd as AG
 from . import metrics as M
-from .backend import B200Backend
+from .backend import B200Backend, is_pinhole_camera
 from .config import CameraOptimizerConfig, HashGridSettings, NeuRADConfig, ScaledCameraOptimizerConfig
 
 _BACKENDS: Dict[int, B200Backend] = {}
@@ -123,7 +123,8 @@ class RayBundle:
 
 
 class Cameras:
-    """cameras/cameras.py (PERSPECTIVE cameras with the AD rolling-shutter metadata): a batch of pinhole cameras whose
+    """cameras/cameras.py with the AD rolling-shutter metadata: a batch of cameras (scene.PinholeCamera descriptors:
+    PERSPECTIVE or FISHEYE, optional k1..k4, p1, p2 distortion, vertical or horizontal shutter) whose
     `generate_rays(camera_indices, keep_shape=True)` returns the full-resolution [H, W] bundle the evaluation loop feeds to
     `get_outputs_for_camera_ray_bundle` (pipelines/ad_pipeline.py:198-208).  One raygen kernel; constant per-image fields
     (sensor index, camera index) are stride-0 views."""
@@ -137,7 +138,9 @@ class Cameras:
 
     def generate_rays(self, camera_indices: int, keep_shape: bool = True) -> RayBundle:
         cam = self.cameras[int(camera_indices)]
-        r = get_backend(self.device).raygen_pinhole(cam)
+        be = get_backend(self.device)
+        # the undistorted perspective model keeps its original entry point; on the device both are raygen_camera_kernel
+        r = be.raygen_pinhole(cam) if is_pinhole_camera(cam) else be.raygen_camera(cam)
         h, w = r["shape"]
         shape = (h, w) if keep_shape else (h * w,)
 

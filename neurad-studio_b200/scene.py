@@ -192,8 +192,10 @@ def make_params_tcnn(cfg: NeuRADConfig, seed: int = 0, table_scale: float = 1.0,
 # ----------------------------------------------------------------------------------------------------------------------
 @dataclass
 class PinholeCamera:
-    """One PERSPECTIVE camera of a `Cameras` batch (cameras/cameras.py) plus the rolling-shutter metadata the AD
-    dataparsers attach (pandaset_dataparser.py:144-146, ad_dataparser.py:361-386)."""
+    """One camera of a `Cameras` batch (cameras/cameras.py) plus the rolling-shutter metadata the AD dataparsers attach
+    (pandaset_dataparser.py:144-146, ad_dataparser.py:361-386).  The defaults are an undistorted PERSPECTIVE camera with a
+    top-to-bottom shutter; ZOD builds "fisheye" cameras with distortion (zod_dataparser.py:226-251), Waymo sets
+    rs_direction "Horizontal" / "Horizontal_reversed" (wod_dataparser.py:129-176)."""
 
     c2w: torch.Tensor  # [3,4], OpenGL convention (camera looks along -z, +y up)
     fx: float
@@ -207,6 +209,9 @@ class PinholeCamera:
     rolling_shutter_time: float = 0.03
     time_to_center_pixel: float = -0.01
     sensor_idx: int = 0
+    camera_type: str = "perspective"  # "perspective" | "fisheye" (CameraType.PERSPECTIVE / FISHEYE)
+    distortion_params: Optional[torch.Tensor] = None  # [6] = k1, k2, k3, k4, p1, p2; None = no distortion
+    rs_direction: str = "Vertical"  # metadata["rs_direction"]: "Vertical" | "Horizontal" | "Horizontal_reversed"
 
 
 @dataclass
