@@ -450,12 +450,15 @@ int b200nerf_lidar_carving_mask(b200nerf_ctx* ctx, const float* bins_e, const ui
 
 /* Kernel variant used by b200nerf_nff_render_fwd:
  *   2 (default) ray-per-lane mapping (a warp = 32 adjacent rays at one sample index: coherent gathers), MLPs on the
- *     wgmma tensor cores with the 3xTF32 split (fp32-level accuracy, |err| ~1e-6 relative);
+ *     wgmma tensor cores with an fp16 three-term hi/lo split of power-of-two scaled operands and fp32 accumulation
+ *     (fp32-level accuracy, |err| ~1e-6 relative);
  *   1 warp-per-ray mapping, wgmma MLPs;   0 warp-per-ray mapping, CUDA-core fp32 FFMA MLPs. */
 int b200nerf_set_mlp_mode(b200nerf_ctx* ctx, int mode);
 
 /* Synchronises with the device and reports (then clears) the device-side failure flag that kernels raise instead
- * of hanging, e.g. when a tensor-core completion barrier times out.  0 = healthy. */
+ * of hanging or returning garbage, e.g. when a tensor-core completion barrier times out, or (code 4) when a main-field
+ * MLP activation of the ray-per-lane kernels reaches 1023.75 in magnitude, beyond their fp16 operand range.
+ * 0 = healthy. */
 int b200nerf_check_status(b200nerf_ctx* ctx);
 
 /* PDFSampler.generate_ray_samples, eval mode, include_original=False (ray_samplers.py:280-361):

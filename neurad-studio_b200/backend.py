@@ -432,8 +432,8 @@ class B200Backend:
 
     def set_mlp_mode(self, mode: str):
         """Kernel variant of render(): 'split' (default) ray-per-lane in two kernels -- sampling at 32 warps/SM, then
-        shading with wgmma MLPs; 'lane' the same code as one fused kernel; 'tc' warp-per-ray + wgmma MLPs
-        (3xTF32); 'ffma' warp-per-ray + CUDA-core fp32 MLPs."""
+        shading with wgmma MLPs (fp16 three-term split); 'lane' the same code as one fused kernel; 'tc' warp-per-ray +
+        wgmma MLPs (3xTF32); 'ffma' warp-per-ray + CUDA-core fp32 MLPs."""
         self._check(self.lib.b200nerf_set_mlp_mode(self._h, {"ffma": 0, "tc": 1, "lane": 2, "split": 3}[mode]))
 
     def set_peer_outputs(self, peer_ptrs: Optional[Dict[str, Sequence[int]]], self_rank: int = -1, row_offset: int = 0):

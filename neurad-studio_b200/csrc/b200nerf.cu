@@ -286,14 +286,15 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
                                                                                       float* __restrict__ scratch,
                                                                                       const float* __restrict__ handoff) {
   extern __shared__ __align__(128) unsigned char smem_shade[];
-  TcShared* tcs = reinterpret_cast<TcShared*>(smem_shade);
+  LaneTcShared* tcs = reinterpret_cast<LaneTcShared*>(smem_shade);
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
-  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads, true);
+  lane_tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
   tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
   MlpLaneTc mlp;
   mlp.t = tcs;
-  mlp.panel_ = reinterpret_cast<float*>(smem_shade + kTcBytes);
+  mlp.panel_ = reinterpret_cast<float*>(smem_shade + kLaneTcBytes);
+  mlp.status = P.status;
   mlp.bar_id = 1 + group;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
   mlp.sh_tcnn = LAYOUT;
@@ -327,14 +328,15 @@ template <bool EDIT>
 __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_render_lane_kernel(const __grid_constant__ RenderParams P,
                                                                           float* __restrict__ scratch) {
   extern __shared__ __align__(128) unsigned char smem_lane[];
-  TcShared* tcs = reinterpret_cast<TcShared*>(smem_lane);
+  LaneTcShared* tcs = reinterpret_cast<LaneTcShared*>(smem_lane);
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), group = warp >> 2;
-  tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads, true);
+  lane_tc_stage_weights(*tcs, P.main_mlp_nn, tid, kLaneThreads);
   tc::fence_async_smem();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
   __syncthreads();
   MlpLaneTc mlp;
   mlp.t = tcs;
-  mlp.panel_ = reinterpret_cast<float*>(smem_lane + kTcBytes);
+  mlp.panel_ = reinterpret_cast<float*>(smem_lane + kLaneTcBytes);
+  mlp.status = P.status;
   mlp.bar_id = 1 + group;
   const LaneScratch sc = lane_scratch_of(scratch, blockIdx.x);
   for (int64_t unit = blockIdx.x; unit < lane_units(P); unit += gridDim.x) {
@@ -2261,6 +2263,10 @@ int b200nerf_check_status(b200nerf_ctx* c) {
   CUDA_TRY(cudaMemcpy(&st, c->d_status, sizeof(int), cudaMemcpyDeviceToHost));
   if (st != 0) {
     cudaMemset(c->d_status, 0, sizeof(int));
+    if (st == kLaneTcRangeStatus)
+      return fail(B200NERF_ERR_CUDA, "device-side failure flag set (code " + std::to_string(st) +
+                                         "): a main-field MLP activation reached the fp16 operand range of the shading "
+                                         "tensor cores (|x| >= 1023.75)");
     return fail(B200NERF_ERR_CUDA, "device-side failure flag set (tensor-core pipeline timed out, code " + std::to_string(st) + ")");
   }
   return 0;

@@ -932,20 +932,20 @@ constexpr int kTcBytes = (sizeof(TcShared) + 127) / 128 * 128;
 // dynamic shared memory of a tensor-core render kernel up to its own part: TcShared, then one stage per warp group
 constexpr size_t tc_smem_bytes(int threads) { return (size_t)kTcBytes + (size_t)(threads / 128) * kTcStageFloats * sizeof(float); }
 NFF_D constexpr int tc_layer_k(int l) { return l == 2 ? 48 : 32; }
+// offset of layer l's hi|lo tiles in TcShared::b (floats) and in LaneTcShared::b (halves, nff_lane.h): 64 K per layer
 NFF_D constexpr int tc_layer_off(int l) { return l == 0 ? 0 : l == 1 ? 2048 : l == 2 ? 4096 : l == 3 ? 7168 : 9216; }
+// where layer l's [32 x K] weights and 32 biases start in the nn.Linear-layout parameters (mlp_geo's last layer: rows 1..32)
+NFF_D constexpr int tc_layer_w(int l) { return l == 0 ? kNnGeoW0 : l == 1 ? kNnGeoW1 + kHidden : l == 2 ? kNnFeatW0 : l == 3 ? kNnFeatW1 : kNnFeatW2; }
+NFF_D constexpr int tc_layer_b(int l) { return l == 0 ? kNnGeoB0 : l == 1 ? kNnGeoB1 + 1 : l == 2 ? kNnFeatB0 : l == 3 ? kNnFeatB1 : kNnFeatB2; }
 
-// cooperative (whole CTA): build the B tiles from the nn.Linear-layout weights in global memory.  `chained`: layers 1-4
-// take their first 32 inputs straight from the previous layer's accumulator fragments (MlpLaneTc, nff_lane.h), so those
-// K rows are permuted (tc::chained_k).
-NFF_D void tc_stage_weights(TcShared& t, const float* NFF_RESTRICT nn, int tid, int nthreads, bool chained = false) {
-  const int w_off[kTcLayers] = {kNnGeoW0, kNnGeoW1 + kHidden /* rows 1..32 */, kNnFeatW0, kNnFeatW1, kNnFeatW2};
-  const int b_off[kTcLayers] = {kNnGeoB0, kNnGeoB1 + 1, kNnFeatB0, kNnFeatB1, kNnFeatB2};
+// cooperative (whole CTA): build the B tiles from the nn.Linear-layout weights in global memory
+NFF_D void tc_stage_weights(TcShared& t, const float* NFF_RESTRICT nn, int tid, int nthreads) {
 #pragma unroll
   for (int l = 0; l < kTcLayers; ++l) {
     const int K = tc_layer_k(l);
     float* hi = t.b + tc_layer_off(l);
-    tc::stage_b_tile(hi, hi + 32 * K, nn + w_off[l], 32, K, 32, K, tid, nthreads, chained && l > 0 ? 32 : 0);
-    for (int i = tid; i < 32; i += nthreads) t.bias[l][i] = nn[b_off[l] + i];
+    tc::stage_b_tile(hi, hi + 32 * K, nn + tc_layer_w(l), 32, K, 32, K, tid, nthreads);
+    for (int i = tid; i < 32; i += nthreads) t.bias[l][i] = nn[tc_layer_b(l) + i];
   }
   for (int i = tid; i < 32; i += nthreads) t.w_sdf[i] = nn[kNnGeoW1 + i];
   if (tid == 0) t.b_sdf = nn[kNnGeoB1];

@@ -349,66 +349,115 @@ struct MlpLaneFfma {
 #if defined(__CUDACC__)
 // Tensor-core version: the tile is the 128 rays of a warp group at this sample index, run as two independent m64 halves
 // (tile rows 64h..64h+63) that each go through all five layers with every activation in wgmma fragment registers:
-//   * layer 0 loads its A fragments straight from the grid-feature panel (rows 0..31; a row pitch of 8 mod 32 banks keeps
+//   * every layer is m64n32k16 wgmma on fp16 operands with fp32 accumulators.  fp32 accuracy comes from the split
+//         a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo        (hi = x rounded to fp16, lo = x - hi rounded to fp16)
+//     three wgmma per k16 step (DESIGN section 4 bounds it);
+//   * the operands are scaled by powers of two to sit inside fp16's range: A by 2^kLaneTcA, layer l's B by 2^e_l, chosen
+//     from the layer's largest weight when the tiles are staged.  Accumulators start at the bias times 2^(kLaneTcA + e_l)
+//     and are scaled back exactly (by 2^-e_l) before ReLU, so the next layer's A is 2^kLaneTcA times the activation;
+//   * layer 0 loads its A fragments straight from the grid-feature panel (rows 0..31; a row pitch of 4 mod 32 banks keeps
 //     those loads free of bank conflicts).  Layer 2's K columns 32..47, the SH encoding of the direction, come from panel
 //     rows 32..47, which the row owner writes next to its features before the group barrier;
-//   * layers 1-4 take the previous layer's accumulator registers as their A operand: their B tiles have the K rows
-//     permuted to match (tc::chained_k), so ReLU and the 3xTF32 hi/lo split work on the same registers;
+//   * layers 1-4 take the previous layer's accumulator registers as their A operand: the fp32 accumulator fragment of an
+//     m64nN wgmma (rows g / g+8, columns 8j+2t, +1) is the register A fragment of an f16 k16 step, pair by pair;
 //   * accumulators start at the bias, layer 4's at bias + geo_embedding (the residual).  geo_embedding waits in the panel
 //     at the thread's own fragment positions (rows 0..31, consumed by layer 0) while layers 2-3 run;
 //   * the sdf neuron is a dot product of layer 0's fragments: 8 terms per thread, then a reduction over the quad;
-//   * one commit and one wait per layer and half, except that layer 2 issues its SH k-steps as a second group after the
-//     geo_embedding ones: as one group its 48 hi/lo operand registers next to the accumulators push the sample loop's
-//     compositing state out to local memory (ptxas: 240 B of spills, against none in the loop this way).  12 waits per
-//     sample.
+//   * one commit and one wait per layer and half: 10 waits per sample;
+//   * an A operand at or beyond fp16's overflow threshold would turn into inf inside the product: each layer checks its
+//     largest scaled operand and raises P.status (kLaneTcRangeStatus) instead.
 // The outputs (feature c of tile row R at panel[c][R], sdf at panel[48][R]) reach the row owner behind the second and
 // last group barrier of the sample.  Panel positions of a tile row are only ever read and written as fragments by the
 // warp whose fragments hold that row, and by the row owner on the far side of a barrier.
-constexpr int kLanePanelPitch = kLaneThreads + 8;
+constexpr int kLanePanelPitch = kLaneThreads + 4;
 constexpr int kLanePanelRows = kGeoIn + kSh + 1;  // grid features | SH | sdf
-constexpr size_t lane_tc_smem_bytes() { return (size_t)kTcBytes + sizeof(float) * kLanePanelRows * kLanePanelPitch; }
+constexpr int kLaneTcA = 6;                       // A operands are 2^6 times the activations: |x| < 1023.75 stays finite
+constexpr float kLaneTcAScale = 64.0f, kLaneTcAUnscale = 1.0f / 64.0f;
+constexpr float kLaneTcOverflow = 65520.0f;       // the smallest fp32 value that rounds to inf in fp16
+constexpr int kLaneTcRangeStatus = 4;             // P.status code: an MLP activation beyond the fp16 operand range
+struct LaneTcShared {
+  __half b[2 * 32 * (32 + 32 + 48 + 32 + 32)];  // hi|lo fp16 B tiles of the 5 layers, layer l times 2^e_l (22 KiB)
+  float bias[kTcLayers][32];                     // times 2^(kLaneTcA + e_l)
+  float up[kTcLayers], down[kTcLayers];          // 2^e_l, 2^-e_l
+  float w_sdf[32];
+  float b_sdf;
+  unsigned wmax[kTcLayers];                      // staging: the bits of the largest |weight| of each layer
+};
+constexpr int kLaneTcBytes = (sizeof(LaneTcShared) + 127) / 128 * 128;
+constexpr size_t lane_tc_smem_bytes() { return (size_t)kLaneTcBytes + sizeof(float) * kLanePanelRows * kLanePanelPitch; }
+
+// cooperative (whole CTA, which it synchronises once): B tiles, scales and biases from the nn.Linear-layout weights.
+// e_l = 15 - (exponent of the layer's largest |weight|, frexp convention): the scaled weights stay below 2^15.
+NFF_D void lane_tc_stage_weights(LaneTcShared& t, const float* NFF_RESTRICT nn, int tid, int nthreads) {
+  if (tid < kTcLayers) t.wmax[tid] = 0u;
+  __syncthreads();
+#pragma unroll
+  for (int l = 0; l < kTcLayers; ++l) {
+    unsigned m = 0u;
+    for (int i = tid; i < 32 * tc_layer_k(l); i += nthreads) m = max(m, __float_as_uint(fabsf(nn[tc_layer_w(l) + i])));
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((tid & 31) == 0 && m) atomicMax(&t.wmax[l], m);
+  }
+  __syncthreads();
+#pragma unroll
+  for (int l = 0; l < kTcLayers; ++l) {
+    int E;
+    frexpf(__uint_as_float(t.wmax[l]), &E);
+    const int e = min(max(15 - E, -60), 60);
+    const float up = __int_as_float((127 + e) << 23), down = __int_as_float((127 - e) << 23);
+    const int K = tc_layer_k(l);
+    __half* hi = t.b + tc_layer_off(l);
+    tc::stage_b_tile_f16(hi, hi + 32 * K, nn + tc_layer_w(l), K, up, tid, nthreads);
+    for (int i = tid; i < 32; i += nthreads) t.bias[l][i] = nn[tc_layer_b(l) + i] * up * kLaneTcAScale;
+    if (tid == 0) t.up[l] = up, t.down[l] = down;
+  }
+  for (int i = tid; i < 32; i += nthreads) t.w_sdf[i] = nn[kNnGeoW1 + i];
+  if (tid == 0) t.b_sdf = nn[kNnGeoB1];
+}
+
 struct MlpLaneTc {
   static constexpr int kPitch = kLanePanelPitch;
-  const TcShared* t;  // B tiles staged by tc_stage_weights(..., chained = true); at the start of dynamic shared memory
-  float* panel_;      // [kLanePanelRows][kPitch] shared memory
-  int bar_id;         // this warp group's named barrier
-  int sh_tcnn = 0;    // 1: tiny-cuda-nn's SphericalHarmonics convention
+  const LaneTcShared* t;  // staged by lane_tc_stage_weights; at the start of dynamic shared memory
+  float* panel_;          // [kLanePanelRows][kPitch] shared memory
+  int* status;            // RenderParams::status
+  int bar_id;             // this warp group's named barrier
+  int sh_tcnn = 0;        // 1: tiny-cuda-nn's SphericalHarmonics convention
   NFF_D float* panel() const { return panel_; }
   NFF_D void group_sync() const { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); }
 
   // Low descriptor word (tc::smem_desc_lo, LBO 128 B) of t->b, taken from the dynamic shared memory symbol rather than
   // from `t`: ptxas then computes it, and every descriptor derived from it, on the uniform datapath.  From the generic
-  // pointer it built all 66 descriptors of a half in per-thread registers and moved each into a uniform register pair
-  // (two R2UR per wgmma; one R2UR per half is left, DESIGN section 4).
+  // pointer it built every descriptor of a half in per-thread registers and moved each into a uniform register pair
+  // (DESIGN section 4).
   NFF_D static uint32_t b_desc_lo() {
     extern __shared__ __align__(128) unsigned char nff_lane_smem[];  // = the kernel's dynamic shared memory
-    return tc::smem_desc_lo(tc::smem_u32(nff_lane_smem + offsetof(TcShared, b)), 128u);
+    return tc::smem_desc_lo(tc::smem_u32(nff_lane_smem + offsetof(LaneTcShared, b)), 128u);
   }
 
-  // acc (this thread's 16 fragment registers of one m64n32 half, preset by the caller) += A * W^T over KS k-steps of a
-  // layer with K inputs, 3xTF32; a = the A fragments, 4 per k-step; OFF = the float offset in t->b of the layer's hi B
-  // tile (lo follows it) from its first k-step on (tc::b_elem_offset: one k-step is 64 floats).  Every descriptor is
-  // b_desc_lo() plus a compile-time constant.
+  // acc (this thread's 16 fragment registers of one m64n32 half, preset by the caller) += A * W^T over the KS k16 steps
+  // of a layer with K inputs; a = the scaled A operands, 8 per k-step in fragment order; OFF = the half offset in t->b of
+  // the layer's hi B tile (lo follows it).  Every descriptor is b_desc_lo() plus a compile-time constant.
   template <int KS, int K, int OFF>
-  NFF_D static void half_mma(float* acc, const float* a) {
+  NFF_D void half_mma(float* acc, const float* a) const {
     uint32_t ah[4 * KS], al[4 * KS];
+    float amax = 0.0f;
 #pragma unroll
     for (int i = 0; i < 4 * KS; ++i) {
-      const float h = tc::tf32_hi(a[i]);
-      ah[i] = __float_as_uint(h);
-      al[i] = __float_as_uint(a[i] - h);
+      amax = fmaxf(amax, fmaxf(fabsf(a[2 * i]), fabsf(a[2 * i + 1])));
+      tc::f16x2_split(a[2 * i], a[2 * i + 1], ah[i], al[i]);
     }
-    constexpr uint32_t sbo = (uint32_t)(K / 4) * 128u;  // (K / 4) core matrices of 128 B per 8-row n block
-    constexpr uint32_t hi_off = (uint32_t)OFF * 4u / 16u, lo_off = (uint32_t)(OFF + 32 * K) * 4u / 16u;
+    if (amax >= kLaneTcOverflow && status) atomicExch(status, kLaneTcRangeStatus);
+    constexpr uint32_t sbo = (uint32_t)(K / 8) * 128u;  // (K / 8) core matrices of 128 B per 8-row n block
+    constexpr uint32_t hi_off = (uint32_t)OFF * 2u / 16u, lo_off = (uint32_t)(OFF + 32 * K) * 2u / 16u;
     const uint32_t b_desc = b_desc_lo();
     tc::wg_fence();
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
       const uint32_t adv = (uint32_t)(ks * 2 * 128) / 16u;  // two 16-byte K-chunks per k-step
       const uint64_t dh = tc::smem_desc_of(b_desc + hi_off + adv, sbo), dl = tc::smem_desc_of(b_desc + lo_off + adv, sbo);
-      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dh);
-      tc::wgmma_tf32<32>(acc, al + 4 * ks, dh);
-      tc::wgmma_tf32<32>(acc, ah + 4 * ks, dl);
+      tc::wgmma_f16_m64n32(acc, ah + 4 * ks, dh);
+      tc::wgmma_f16_m64n32(acc, al + 4 * ks, dh);
+      tc::wgmma_f16_m64n32(acc, ah + 4 * ks, dl);
     }
     tc::wg_commit();
     tc::wg_wait<0>();
@@ -417,25 +466,19 @@ struct MlpLaneTc {
 #pragma unroll
     for (int i = 0; i < 4 * KS; ++i) asm volatile("" : "+r"(ah[i]), "+r"(al[i])::"memory");
   }
-  // A fragments of k-steps [0, 4) from the accumulator fragments of the previous layer (K rows of B permuted)
-  NFF_D static void chain(float* a, const float* acc) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      a[4 * j + 0] = acc[4 * j + 0];
-      a[4 * j + 1] = acc[4 * j + 2];
-      a[4 * j + 2] = acc[4 * j + 1];
-      a[4 * j + 3] = acc[4 * j + 3];
-    }
-  }
-  // A fragments of k-steps [ks0, ks0 + n) from panel rows 8 ks0 .. (p = the panel at this thread's fragment row g)
+  // scaled A operands of k16 steps [ks0, ks0 + n) from panel rows 16 ks0 .. (p = the panel at this thread's fragment row g)
   NFF_D static void load_a(float* a, const float* p, int q, int ks0, int n) {
 #pragma unroll
     for (int i = 0; i < n; ++i) {
-      const float* r = p + (8 * (ks0 + i) + q) * kPitch;
-      a[4 * i + 0] = r[0];
-      a[4 * i + 1] = r[8];
-      a[4 * i + 2] = r[4 * kPitch];
-      a[4 * i + 3] = r[4 * kPitch + 8];
+      const float* r = p + (16 * (ks0 + i) + 2 * q) * kPitch;
+      a[8 * i + 0] = r[0] * kLaneTcAScale;
+      a[8 * i + 1] = r[kPitch] * kLaneTcAScale;
+      a[8 * i + 2] = r[8] * kLaneTcAScale;
+      a[8 * i + 3] = r[kPitch + 8] * kLaneTcAScale;
+      a[8 * i + 4] = r[8 * kPitch] * kLaneTcAScale;
+      a[8 * i + 5] = r[9 * kPitch] * kLaneTcAScale;
+      a[8 * i + 6] = r[8 * kPitch + 8] * kLaneTcAScale;
+      a[8 * i + 7] = r[9 * kPitch + 8] * kLaneTcAScale;
     }
   }
   NFF_D static void bias_init(float* acc, const float* bias, int q) {
@@ -445,6 +488,11 @@ struct MlpLaneTc {
       acc[4 * j + 0] = acc[4 * j + 2] = b.x;
       acc[4 * j + 1] = acc[4 * j + 3] = b.y;
     }
+  }
+  // accumulators times 2^-e_l: 2^kLaneTcA times the layer's output (exact)
+  NFF_D static void unscale(float* acc, float down) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i] *= down;
   }
   NFF_D static void relu(float* acc) {
 #pragma unroll
@@ -466,11 +514,12 @@ struct MlpLaneTc {
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
       float* const p = fr + 64 * h;
-      float a[16], acc[16];
+      float a[24], acc[16];
       // layer 0: grid features -> hidden, ReLU, sdf
-      load_a(a, p, q, 0, 4);
+      load_a(a, p, q, 0, 2);
       bias_init(acc, t->bias[0], q);
-      half_mma<4, 32, tc_layer_off(0)>(acc, a);
+      half_mma<2, 32, tc_layer_off(0)>(acc, a);
+      unscale(acc, t->down[0]);
       relu(acc);
       float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
@@ -483,14 +532,16 @@ struct MlpLaneTc {
       s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
       s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
       s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-      if (q == 0) {
-        p[(kGeoIn + kSh) * kPitch] = s0 + t->b_sdf;
-        p[(kGeoIn + kSh) * kPitch + 8] = s1 + t->b_sdf;
+      if (q == 0) {  // the sums of the scaled activations are exactly 2^kLaneTcA times those of the activations
+        p[(kGeoIn + kSh) * kPitch] = s0 * kLaneTcAUnscale + t->b_sdf;
+        p[(kGeoIn + kSh) * kPitch + 8] = s1 * kLaneTcAUnscale + t->b_sdf;
       }
-      // layer 1: -> geo_embedding, parked at this thread's fragment positions of panel rows 0..31
-      chain(a, acc);
+      // layer 1: -> geo_embedding (scaled), parked at this thread's fragment positions of panel rows 0..31
+#pragma unroll
+      for (int i = 0; i < 16; ++i) a[i] = acc[i];
       bias_init(acc, t->bias[1], q);
-      half_mma<4, 32, tc_layer_off(1)>(acc, a);
+      half_mma<2, 32, tc_layer_off(1)>(acc, a);
+      unscale(acc, t->down[1]);
       __syncwarp();  // the warp's layer-0 fragment loads of these rows are done
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -498,30 +549,37 @@ struct MlpLaneTc {
         r[0] = acc[4 * j + 0], r[kPitch] = acc[4 * j + 1], r[8] = acc[4 * j + 2], r[kPitch + 8] = acc[4 * j + 3];
       }
       // layer 2: [geo_embedding | SH] -> hidden, ReLU
-      chain(a, acc);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) a[i] = acc[i];
+      load_a(a + 16, p, q, 2, 1);
       bias_init(acc, t->bias[2], q);
-      half_mma<4, 48, tc_layer_off(2)>(acc, a);
-      load_a(a, p, q, 4, 2);
-      half_mma<2, 48, tc_layer_off(2) + 4 * 64>(acc, a);
+      half_mma<3, 48, tc_layer_off(2)>(acc, a);
+      unscale(acc, t->down[2]);
       relu(acc);
       // layer 3: hidden -> hidden, ReLU
-      chain(a, acc);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) a[i] = acc[i];
       bias_init(acc, t->bias[3], q);
-      half_mma<4, 32, tc_layer_off(3)>(acc, a);
+      half_mma<2, 32, tc_layer_off(3)>(acc, a);
+      unscale(acc, t->down[3]);
       relu(acc);
       // layer 4: hidden -> features, accumulated onto bias + geo_embedding; out to the same positions
-      chain(a, acc);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) a[i] = acc[i];
       bias_init(acc, t->bias[4], q);
+      const float up4 = t->up[4], out4 = t->down[4] * kLaneTcAUnscale;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float* r = p + (8 * j + 2 * q) * kPitch;
-        acc[4 * j + 0] += r[0], acc[4 * j + 1] += r[kPitch], acc[4 * j + 2] += r[8], acc[4 * j + 3] += r[kPitch + 8];
+        acc[4 * j + 0] += r[0] * up4, acc[4 * j + 1] += r[kPitch] * up4;
+        acc[4 * j + 2] += r[8] * up4, acc[4 * j + 3] += r[kPitch + 8] * up4;
       }
-      half_mma<4, 32, tc_layer_off(4)>(acc, a);
+      half_mma<2, 32, tc_layer_off(4)>(acc, a);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         float* r = p + (8 * j + 2 * q) * kPitch;
-        r[0] = acc[4 * j + 0], r[kPitch] = acc[4 * j + 1], r[8] = acc[4 * j + 2], r[kPitch + 8] = acc[4 * j + 3];
+        r[0] = acc[4 * j + 0] * out4, r[kPitch] = acc[4 * j + 1] * out4;
+        r[8] = acc[4 * j + 2] * out4, r[kPitch + 8] = acc[4 * j + 3] * out4;
       }
     }
     group_sync();  // every tile row's outputs are in

@@ -8,6 +8,7 @@
 //     x*w ~= x_hi*w_hi + x_lo*w_hi + x_hi*w_lo        (x_hi = x with the 13 low mantissa bits cleared)
 // i.e. three wgmma per 8-wide k-step accumulating into the same registers; the dropped x_lo*w_lo term is ~2^-22 relative.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -111,6 +112,14 @@ __device__ __forceinline__ void wgmma_bf16_m64n128(float* d, uint64_t a_desc, ui
                : TC_D32(0), TC_D32(32)
                : "l"(a_desc), "l"(b_desc), "r"(1));
 }
+// m64n32k16 with fp16 operands and fp32 accumulators; A = this thread's 4 f16x2 fragment registers (row g / g+8,
+// k 2t, 2t+1 / 2t+8, 2t+9; the lower k in the low half), B from a K-major descriptor.
+__device__ __forceinline__ void wgmma_f16_m64n32(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+               : TC_D16(0)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+}
 template <int N>
 __device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t b_desc) {
   static_assert(N == 16 || N == 32 || N == 48 || N == 64, "tf32 tile widths");
@@ -130,22 +139,44 @@ __device__ __forceinline__ uint32_t b_elem_offset(int n, int k, int k_pad) {
 }
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
-// Input column of B row k when the A operand is the previous layer's accumulator fragment taken as is: a thread holds
-// D columns 8j+2t, 8j+2t+1 and the TF32 A fragment wants columns 8j+t, 8j+t+4, so the K rows of each 8-wide chunk are
-// permuted to match (p < 4: column 2p; p >= 4: column 2(p-4)+1).
-__host__ __device__ constexpr int chained_k(int k) { return (k & ~7) | ((k & 7) < 4 ? 2 * (k & 7) : 2 * (k & 7) - 7); }
-
-// cooperative: all `nthreads` threads of the CTA.  The first `k_chained` K rows are permuted by chained_k.
+// cooperative: all `nthreads` threads of the CTA
 __device__ __forceinline__ void stage_b_tile(float* hi, float* lo, const float* __restrict__ w, int n_real, int k_real, int n_pad,
-                                             int k_pad, int tid, int nthreads, int k_chained = 0) {
+                                             int k_pad, int tid, int nthreads) {
   for (int i = tid; i < n_pad * k_pad; i += nthreads) {
     int n = i / k_pad, k = i % k_pad;
-    const int kw = k < k_chained ? chained_k(k) : k;
-    float v = (n < n_real && kw < k_real) ? w[n * k_real + kw] : 0.0f;
+    float v = (n < n_real && k < k_real) ? w[n * k_real + k] : 0.0f;
     float h = tf32_hi(v);
     uint32_t off = b_elem_offset(n, k, k_pad);
     hi[off] = h;
     lo[off] = v - h;  // exact in fp32; the tensor core truncates it to TF32 (error ~2^-22 |v|)
+  }
+}
+
+// fp16 hi/lo split of a pair: hi = (x0, x1) rounded to fp16, lo = the remainders x - hi (exact in fp32) rounded to fp16.
+// x0 goes to the low half of each register.  FP16 has TF32's 11 significant bits, so hi + lo carries 22 of them.
+__device__ __forceinline__ void f16x2_split(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+// fp16 B tile, canonical K-major no-swizzle layout for k16 steps: 8-row x 16-byte core matrices (8 halves along K), core
+// (nb, kc) at nb*SBO + kc*LBO with LBO = 128 B, SBO = (K_pad/8)*128 B; element (n,k) at +(n%8)*16 B + (k%8)*2 B.
+__device__ __forceinline__ uint32_t b_elem_offset_f16(int n, int k, int k_pad) {
+  return (uint32_t)((n >> 3) * (k_pad >> 3) * 64 + (k >> 3) * 64 + (n & 7) * 8 + (k & 7));  // in halves
+}
+// cooperative (all `nthreads` threads of the CTA): W[n_real x k_real] (row major, fp32) times `scale` (a power of two)
+// -> fp16 hi / lo tiles [32 x k_real]
+__device__ __forceinline__ void stage_b_tile_f16(__half* hi, __half* lo, const float* __restrict__ w, int k_real, float scale,
+                                                 int tid, int nthreads) {
+  for (int i = tid; i < 32 * k_real; i += nthreads) {
+    const int n = i / k_real, k = i % k_real;
+    const float v = w[i] * scale;
+    const __half h = __float2half_rn(v);
+    const uint32_t off = b_elem_offset_f16(n, k, k_real);
+    hi[off] = h;
+    lo[off] = __float2half_rn(v - __half2float(h));
   }
 }
 // 64-bit shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),

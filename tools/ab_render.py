@@ -8,7 +8,8 @@ Each build runs in its own child process, loaded through NFF_LIB as tools/perf_p
   nears_fars   the first camera image with per-ray nears / fars (round 0 computes its edges per ray)
 untraced (all outputs) and traced (the proposal stage on every 16th ray: weights, edges, indices, actor ids; once with
 actor ids, which turns the early exit off, and once without).  The parent compares every array of the two builds with
-np.array_equal and byte for byte, then prints the median and range of the per-render device time (CUDA events) of each
+np.array_equal and byte for byte (and prints, for an array that differs, its largest difference over its largest
+magnitude), then prints the median and range of the per-render device time (CUDA events) of each
 build and scene (config2_traced: the full config-2 step with the proposal trace but no actor ids), over R rounds that
 alternate the builds, K renders each.  Exit code 1 if any array differs.
 """
@@ -153,6 +154,10 @@ def main() -> int:
                     diff = [k for k in A.files if not (np.array_equal(A[k], B[k]) and A[k].tobytes() == B[k].tobytes())]
                     bad += len(diff)
                     print(f"{s}: {len(A.files)} arrays compared, {'all identical' if not diff else 'DIFFERENT: ' + ', '.join(diff)}")
+                    for k in diff:  # max |old - new| over max |old|, the tensor's scale
+                        a64, b64 = A[k].astype(np.float64), B[k].astype(np.float64)
+                        scale = np.nanmax(np.abs(a64)) if a64.size else 0.0
+                        print(f"    {k}: max |old - new| / max |old| = {np.nanmax(np.abs(a64 - b64)) / max(scale, 1e-30):.3g}")
                     os.remove(os.path.join(dirs["old"], f"{s}.npz"))
                     os.remove(os.path.join(dirs["new"], f"{s}.npz"))
     print(f"device: {device}; per-render device time over {a.rounds} alternated rounds x {a.reps} renders")
