@@ -641,6 +641,52 @@ int b200nerf_raygen_lidar_grid(b200nerf_ctx* ctx, const float* l2w_host, float e
                                float revolution_time, const float* velocity_host, float h_div, float v_div,
                                float* origins, float* directions, float* pixel_area, float* times, void* stream);
 
+/* ---- lidar simulation ----------------------------------------------------------------------------------- */
+
+/* One simulated sweep of a spinning lidar: the nominal sensor pose at the scan time and the sensor's rolling-shutter and
+ * beam-footprint parameters.  An array of these lives in device memory. */
+typedef struct b200nerf_lidar_sweep {
+  float l2w[12];         /* sensor-to-world 3x4 row major at scan_time */
+  float scan_time;
+  float revolution_time; /* 0: every ray at scan_time from the nominal origin */
+  float velocity[3];     /* world frame, read only when has_velocity != 0 */
+  int has_velocity;
+  float h_div, v_div;    /* beam divergences: pixel_area = h_div * v_div */
+  int sensor_idx;        /* appearance-embedding row of the sensor */
+  int pad_;
+} b200nerf_lidar_sweep;
+
+/* Beam x column ray grids of n_sweeps sweeps of one shape (beams x n_azimuth) in one launch: ray i = ((s * beams) + b) *
+ * n_azimuth + k.  Beam b of sweep s points at elevation elevations[s * beams + b] (radians, any order and spacing) and
+ * azimuth float(k * azimuth_step) + azimuth_offsets[s * beams + b] (offsets NULL = 0); its time offset is that of the
+ * rotor column, dt = (float(k * azimuth_step) / 2pi - 0.5) * revolution_time, with origin l2w.t + velocity * dt as in
+ * b200nerf_raygen_lidar_grid, which is the same kernel with one sweep and linspace elevations.  Optional outputs (NULL to
+ * skip): sensor_idx [N] (int64), is_lidar [N] (uint8, 1), index [N, 3] (int32 sweep, beam, column).  `sweeps`,
+ * `elevations` and `azimuth_offsets` are device arrays. */
+int b200nerf_raygen_lidar_sweeps(b200nerf_ctx* ctx, const b200nerf_lidar_sweep* sweeps, int n_sweeps, int beams,
+                                 int n_azimuth, double azimuth_step_rad, const float* elevations,
+                                 const float* azimuth_offsets, float* origins, float* directions, float* pixel_area,
+                                 float* times, int64_t* sensor_idx, uint8_t* is_lidar, int* index, void* stream);
+
+/* The point clouds of rendered sweeps (the viewer's lidar render, viewer/render_state_machine.py:416-430, with the
+ * sensor-frame transform of models/ad_model.py:107-113).  For the N = n_sweeps * rays_per_sweep rays of
+ * b200nerf_raygen_lidar_sweeps, rendered to depth / intensity (and ray_drop_prob when use_ray_drop):
+ *   kept  = use_ray_drop ? ray_drop_prob < threshold : depth < threshold
+ *   world = origin + direction * depth,  sensor = pose_inverse(sweeps[s].l2w) (world, 1),  dt = time - scan_time
+ * Kept rays are written in ray order (sweep, beam, column row major, the order of a boolean index) at the rows a
+ * device-wide exclusive scan gives them: points_sensor [N, 5] = (x, y, z, intensity, dt), points_world [N, 3], index
+ * [N, 3] int32 (sweep, beam, column); rows past the kept count are left untouched.  counts [n_sweeps + 1] (device,
+ * int32) = kept rays per sweep, then their total; offsets [n_sweeps] = each sweep's first row.  No atomics: the
+ * output is deterministic.  No host synchronisation and no allocation; the workspace holds at least
+ * b200nerf_lidar_sweep_workspace_bytes(n_sweeps, rays_per_sweep) bytes.  A non-finite threshold, n_sweeps < 1 or
+ * rays_per_sweep < 1 returns B200NERF_ERR_INVALID. */
+size_t b200nerf_lidar_sweep_workspace_bytes(int n_sweeps, int64_t rays_per_sweep);
+int b200nerf_lidar_sweep_points(b200nerf_ctx* ctx, const b200nerf_lidar_sweep* sweeps, int n_sweeps, int beams,
+                                int n_azimuth, const float* origins, const float* directions, const float* times,
+                                const float* depth, const float* intensity, const float* ray_drop_prob, int use_ray_drop,
+                                float threshold, float* points_sensor, float* points_world, int* index, int* counts,
+                                int* offsets, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- lidar evaluation ----------------------------------------------------------------------------------- */
 
 /* Chamfer distance of NeuRAD's lidar metrics (utils/math.py:745-798, models/neurad.py:614-618): src [n_src, src_stride]

@@ -7,5 +7,6 @@ from .config import (HashGridSettings, NeuRADConfig, NeuRADHashEncodingConfig, P
                      small_config)
 from .metrics import chamfer_distance  # noqa: F401
 from .metrics import ssim as structural_similarity_index_measure  # noqa: F401
+from .scene import LidarSensor  # noqa: F401
 
 __version__ = "0.1.0"

@@ -5,6 +5,7 @@ is in libb200nerf.so.  There is no CPU path: constructing a `B200Backend` withou
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 from typing import Dict, Optional, Sequence, Tuple
 
@@ -68,6 +69,16 @@ def camera_descriptor(cam) -> "_lib.Camera":
     d.rolling_shutter_time, d.time_to_center_pixel = cam.rolling_shutter_time, cam.time_to_center_pixel
     d.rs_direction = _lib.RS_DIRECTIONS[rs_direction]
     return d
+
+
+def lidar_columns(azim_res_deg: float) -> Tuple[float, int]:
+    """(step in radians, column count) of the viewer's `torch.arange(0, 2 pi, np.deg2rad(azim_res_deg))`."""
+    import numpy as np
+
+    step = float(np.deg2rad(azim_res_deg))
+    if not (math.isfinite(step) and step > 0.0):
+        raise ValueError(f"azimuth resolution must be finite and positive, got {azim_res_deg}")
+    return step, int(math.ceil((2 * math.pi) / step))  # len(torch.arange(0, 2*pi, step))
 
 
 def grid_desc(g: HashGridSettings, scalings: Optional[torch.Tensor] = None) -> GridDesc:
@@ -1014,12 +1025,9 @@ class B200Backend:
                           scan_time: float, revolution_time: float = 0.1, velocity: Optional[torch.Tensor] = None,
                           out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
         """Beam x azimuth lidar grid with rolling shutter (BASELINE config 4 input: 128 beams x 2048 azimuths)."""
-        import math
-
         import numpy as np
 
-        step = float(np.deg2rad(azim_res_deg))
-        n_az = int(math.ceil((2 * math.pi) / step))  # len(torch.arange(0, 2*pi, step))
+        step, n_az = lidar_columns(azim_res_deg)
         n = beams * n_az
         o, d, a, t = self._ray_buffers(n, out)
         cl2w = (ctypes.c_float * 12)(*l2w.reshape(-1).tolist())
@@ -1030,6 +1038,108 @@ class B200Backend:
                                                 3.0e-3, 1.5e-3, _ptr(o), _ptr(d), _ptr(a), _ptr(t), self._stream)
         )
         return {"origins": o, "directions": d, "pixel_area": a, "times": t, "shape": (beams, n_az)}
+
+    def raygen_lidar_sweeps(self, sensors, poses: torch.Tensor, times, velocities=None) -> Dict[str, torch.Tensor]:
+        """Rays of S simulated sweeps in one launch (b200nerf_raygen_lidar_sweeps): `sensors` is one scene.LidarSensor or
+        one per sweep, all with the same beam count and azimuth resolution; poses [S,3,4] (or [S,4,4]) sensor-to-world at
+        the scan times; times [S]; velocities [S,3] or None (no origin motion).  Returns the flat ray buffers of the
+        render (origins, directions, pixel_area, times, sensor_idx int64, is_lidar uint8), index [N,3] int32 (sweep,
+        beam, column), `sweeps` (the device descriptors the point epilogue reads) and shape (S, beams, columns).
+
+        The description is host data: it is validated on the host and uploaded without a host wait.  Poses, times or
+        tables passed as CUDA tensors are read back to the host first, which waits on the device."""
+        poses = torch.as_tensor(poses, dtype=torch.float32).cpu()
+        if poses.dim() == 2:
+            poses = poses[None]
+        if poses.dim() != 3 or poses.shape[-2] not in (3, 4) or poses.shape[-1] != 4:
+            raise ValueError(f"poses must be [S, 3, 4] or [S, 4, 4] sensor-to-world matrices, got {tuple(poses.shape)}")
+        n_sw = poses.shape[0]
+        times = torch.as_tensor(times, dtype=torch.float32).cpu().reshape(-1)
+        sensors = list(sensors) if isinstance(sensors, (list, tuple)) else [sensors] * n_sw
+        vel = None if velocities is None else torch.as_tensor(velocities, dtype=torch.float32).cpu().reshape(-1, 3)
+        if n_sw < 1 or times.numel() != n_sw or len(sensors) != n_sw or (vel is not None and vel.shape[0] != n_sw):
+            raise ValueError(f"{n_sw} poses need as many times, sensors and velocities (got {times.numel()}, {len(sensors)}, "
+                             f"{None if vel is None else vel.shape[0]})")
+        elev = [torch.as_tensor(s_.elevations, dtype=torch.float32).cpu().reshape(-1) for s_ in sensors]
+        beams = elev[0].numel()
+        res = float(sensors[0].azimuth_resolution_deg)
+        if beams < 1 or any(e.numel() != beams for e in elev) or any(float(s_.azimuth_resolution_deg) != res for s_ in sensors):
+            raise ValueError("every sweep of one call needs a non-empty beam table of one size and one azimuth resolution")
+        step, n_az = lidar_columns(res)
+        off = [torch.zeros(beams) if s_.azimuth_offsets is None else torch.as_tensor(s_.azimuth_offsets, dtype=torch.float32).cpu().reshape(-1)
+               for s_ in sensors]
+        if any(o.numel() != beams for o in off):
+            raise ValueError("azimuth_offsets must hold one value per beam")
+        elev, off = torch.stack(elev), torch.stack(off)
+        desc = (_lib.LidarSweep * n_sw)()
+        for i, s_ in enumerate(sensors):
+            d = desc[i]
+            d.l2w[:] = poses[i, :3].reshape(-1).tolist()
+            d.scan_time, d.revolution_time = float(times[i]), float(s_.revolution_time)
+            d.h_div, d.v_div, d.sensor_idx = float(s_.h_div), float(s_.v_div), int(s_.sensor_idx)
+            if vel is not None:
+                d.velocity[:] = vel[i].tolist()
+                d.has_velocity = 1
+            scal = list(d.l2w) + [d.scan_time, d.revolution_time, d.h_div, d.v_div] + list(d.velocity)
+            if not all(math.isfinite(v) for v in scal):
+                raise ValueError(f"sweep {i}: pose, time, velocity, revolution time and divergences must be finite")
+        if not (torch.isfinite(elev).all() and torch.isfinite(off).all()):
+            raise ValueError("beam tables must be finite")
+        # descriptors, elevations and (when any is non-zero) offsets go up in one copy from pinned memory that does not
+        # wait on the host: the caching host allocator keeps the staging block until the copy has run
+        has_off = bool(off.any())
+        n_desc, n_tab = ctypes.sizeof(desc), 4 * n_sw * beams
+        stage = torch.empty(n_desc + n_tab * (2 if has_off else 1), dtype=torch.uint8, pin_memory=True)
+        stage[:n_desc].copy_(torch.frombuffer(bytearray(bytes(desc)), dtype=torch.uint8))
+        stage[n_desc:n_desc + n_tab].view(torch.float32).copy_(elev.reshape(-1))
+        if has_off:
+            stage[n_desc + n_tab:].view(torch.float32).copy_(off.reshape(-1))
+        staged = stage.to(self.device, non_blocking=True)
+        base = staged.data_ptr()
+        sweeps = staged[:n_desc]
+        elev_p = ctypes.c_void_p(base + n_desc)
+        off_p = ctypes.c_void_p(base + n_desc + n_tab) if has_off else None
+        n = n_sw * beams * n_az
+        o, d_, a, t = self._ray_buffers(n, None)
+        sensor_idx = torch.empty(n, 1, dtype=torch.int64, device=self.device)
+        is_lidar = torch.empty(n, 1, dtype=torch.uint8, device=self.device)
+        index = torch.empty(n, 3, dtype=torch.int32, device=self.device)
+        self._check(self.lib.b200nerf_raygen_lidar_sweeps(
+            self._h, _ptr(sweeps), n_sw, beams, n_az, step, elev_p, off_p, _ptr(o), _ptr(d_), _ptr(a), _ptr(t),
+            _ptr(sensor_idx), _ptr(is_lidar), _ptr(index), self._stream))
+        return {"origins": o, "directions": d_, "pixel_area": a, "times": t, "sensor_idx": sensor_idx,
+                "is_lidar": is_lidar.view(torch.bool), "index": index, "sweeps": sweeps, "shape": (n_sw, beams, n_az)}
+
+    def lidar_sweep_points(self, rays: Dict[str, torch.Tensor], depth: torch.Tensor, intensity: torch.Tensor,
+                           ray_drop_prob: Optional[torch.Tensor], threshold: float) -> Dict[str, torch.Tensor]:
+        """The point epilogue of rendered sweeps (b200nerf_lidar_sweep_points) for the rays of `raygen_lidar_sweeps`:
+        kept = ray_drop_prob < threshold, or depth < threshold when ray_drop_prob is None.  Returns capacity-sized [N, ...]
+        buffers points_sensor [N,5] (x, y, z, intensity, dt in the sweep's sensor frame), points_world [N,3], index [N,3]
+        int32, whose first counts[-1] rows hold the kept rays in (sweep, beam, column) order, and counts [S+1] /
+        offsets [S] int32 on the device.  Nothing synchronises the host."""
+        n_sw, beams, n_az = rays["shape"]
+        n = n_sw * beams * n_az
+
+        def col(t):
+            t = self._dev(t.detach().reshape(-1))
+            if t.numel() != n:
+                raise ValueError(f"lidar sweep points: {t.numel()} values for {n} rays")
+            return t
+
+        dep, inten = col(depth), col(intensity)
+        prob = None if ray_drop_prob is None else col(ray_drop_prob)
+        ps = torch.empty(n, 5, device=self.device)
+        pw = torch.empty(n, 3, device=self.device)
+        index = torch.empty(n, 3, dtype=torch.int32, device=self.device)
+        counts = torch.empty(n_sw + 1, dtype=torch.int32, device=self.device)
+        offsets = torch.empty(n_sw, dtype=torch.int32, device=self.device)
+        ws = torch.empty(max(int(self.lib.b200nerf_lidar_sweep_workspace_bytes(n_sw, beams * n_az)), 16), dtype=torch.uint8,
+                         device=self.device)
+        self._check(self.lib.b200nerf_lidar_sweep_points(
+            self._h, _ptr(rays["sweeps"]), n_sw, beams, n_az, _ptr(rays["origins"]), _ptr(rays["directions"]),
+            _ptr(rays["times"]), _ptr(dep), _ptr(inten), _ptr(prob), int(prob is not None), float(threshold), _ptr(ps),
+            _ptr(pw), _ptr(index), _ptr(counts), _ptr(offsets), _ptr(ws), ws.numel(), self._stream))
+        return {"points_sensor": ps, "points_world": pw, "index": index, "counts": counts, "offsets": offsets}
 
     # ------------------------------------------------------------------------------------------ lidar evaluation
     def chamfer_distance(self, pred: torch.Tensor, gt: torch.Tensor, normalize_with_target: bool = True,

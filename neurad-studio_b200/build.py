@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libb200nerf.so")
 SOURCES = ["b200nerf.cu"]
-HEADERS = ["nff_device.h", "nff_lane.h", "tc_mlp.cuh", "rgb_decoder.cuh", "nff_modules.h", "modules.cuh", "nff_params.h", "simt.h", "lidar_eval.cuh", "lidar_loss.cuh", "image_metrics.cuh", "camera_rays.h", os.path.join("..", "..", "include", "b200nerf.h")]
+HEADERS = ["nff_device.h", "nff_lane.h", "tc_mlp.cuh", "rgb_decoder.cuh", "nff_modules.h", "modules.cuh", "nff_params.h", "simt.h", "lidar_eval.cuh", "lidar_loss.cuh", "image_metrics.cuh", "camera_rays.h", "lidar_sim.cuh", os.path.join("..", "..", "include", "b200nerf.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",

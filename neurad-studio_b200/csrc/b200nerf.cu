@@ -16,6 +16,7 @@
 #include "lidar_loss.cuh"
 #include "image_metrics.cuh"
 #include "camera_rays.h"
+#include "lidar_sim.cuh"
 
 using namespace nff;
 
@@ -940,6 +941,8 @@ __global__ void raygen_lidar_kernel(LidarArgs a, const float* __restrict__ pts, 
 // Beam x azimuth lidar ray grid (viewer/render_state_machine.py:395-407: d = (cos v cos h, cos v sin h, sin v) over
 // linspace elevations x arange azimuths) with a rolling-shutter sweep: per-ray time offset linear in azimuth over one
 // revolution and origin shifted by velocity * dt (cameras/lidars.py:421-423, 625-639).  BASELINE config 4's input shape.
+// With `sweeps` set, blockIdx.y's sweep reads its pose, time, velocity and footprint from sweeps[s] and its beams from
+// the elevation / azimuth-offset tables; the fields above `sweeps` then only give the grid shape.
 struct LidarGridArgs {
   float l2w[12];
   float elev0, elev1;   // radians
@@ -947,36 +950,75 @@ struct LidarGridArgs {
   int beams, n_az;
   float scan_time, rev_time, vel[3], h_div, v_div;
   int has_vel;
+  const b200nerf_lidar_sweep* sweeps;  // device, one per blockIdx.y; NULL: one sweep described by the fields above
+  const float* elev;                   // device [sweeps, beams] (with `sweeps`)
+  const float* az_off;                 // device [sweeps, beams] or NULL
+  int64_t* sensor_idx;                 // optional outputs
+  uint8_t* is_lidar;
+  int* index;
 };
 __global__ void raygen_lidar_grid_kernel(LidarGridArgs a, float* __restrict__ origins, float* __restrict__ dirs,
                                          float* __restrict__ area, float* __restrict__ times) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (int64_t)a.beams * a.n_az) return;
-  const int b = (int)(i / a.n_az), k = (int)(i % a.n_az);
-  // torch.linspace(e0, e1, beams): start + step*i for the first half, end - step*(n-1-i) for the second
-  const float step = a.beams > 1 ? fdiv(fsub(a.elev1, a.elev0), (float)(a.beams - 1)) : 0.f;
-  const float v = b < a.beams / 2 ? fadd(a.elev0, fmul(step, (float)b)) : fsub(a.elev1, fmul(step, (float)(a.beams - 1 - b)));
+  const int64_t per = (int64_t)a.beams * a.n_az;
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= per) return;
+  const int s = blockIdx.y;
+  const int64_t i = s * per + j;
+  const int b = (int)(j / a.n_az), k = (int)(j % a.n_az);
+  float l2w[12], vel[3], scan_time, rev_time, h_div, v_div;
+  int has_vel;
+  if (a.sweeps) {
+    const b200nerf_lidar_sweep& w = a.sweeps[s];
+#pragma unroll
+    for (int r = 0; r < 12; ++r) l2w[r] = w.l2w[r];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) vel[r] = w.velocity[r];
+    scan_time = w.scan_time, rev_time = w.revolution_time, h_div = w.h_div, v_div = w.v_div, has_vel = w.has_velocity;
+  } else {
+#pragma unroll
+    for (int r = 0; r < 12; ++r) l2w[r] = a.l2w[r];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) vel[r] = a.vel[r];
+    scan_time = a.scan_time, rev_time = a.rev_time, h_div = a.h_div, v_div = a.v_div, has_vel = a.has_vel;
+  }
+  float v;
+  if (a.sweeps) {
+    v = a.elev[(int64_t)s * a.beams + b];
+  } else {
+    // torch.linspace(e0, e1, beams): start + step*i for the first half, end - step*(n-1-i) for the second
+    const float step = a.beams > 1 ? fdiv(fsub(a.elev1, a.elev0), (float)(a.beams - 1)) : 0.f;
+    v = b < a.beams / 2 ? fadd(a.elev0, fmul(step, (float)b)) : fsub(a.elev1, fmul(step, (float)(a.beams - 1 - b)));
+  }
+  // the rotor column's azimuth sets the time; the beam points at it plus its own offset
   const float h = (float)((double)k * a.az_step);
-  const float cv = cosf(v), sv = sinf(v), ch = cosf(h), sh = sinf(h);
+  const float hb = a.az_off ? fadd(h, a.az_off[(int64_t)s * a.beams + b]) : h;
+  const float cv = cosf(v), sv = sinf(v), ch = cosf(hb), sh = sinf(hb);
   const float dl[3] = {fmul(cv, ch), fmul(cv, sh), sv};
   float d[3], o[3];
 #pragma unroll
   for (int r = 0; r < 3; ++r) {
-    d[r] = fadd(fadd(fmul(a.l2w[4 * r], dl[0]), fmul(a.l2w[4 * r + 1], dl[1])), fmul(a.l2w[4 * r + 2], dl[2]));
-    o[r] = a.l2w[4 * r + 3];
+    d[r] = fadd(fadd(fmul(l2w[4 * r], dl[0]), fmul(l2w[4 * r + 1], dl[1])), fmul(l2w[4 * r + 2], dl[2]));
+    o[r] = l2w[4 * r + 3];
   }
-  const float dt = fmul(fsub(fdiv(h, 6.283185307179586f), 0.5f), a.rev_time);
-  if (a.has_vel) {
+  const float dt = fmul(fsub(fdiv(h, 6.283185307179586f), 0.5f), rev_time);
+  if (has_vel) {
 #pragma unroll
-    for (int r = 0; r < 3; ++r) o[r] = fadd(o[r], fmul(dt, a.vel[r]));
+    for (int r = 0; r < 3; ++r) o[r] = fadd(o[r], fmul(dt, vel[r]));
   }
 #pragma unroll
   for (int r = 0; r < 3; ++r) {
     origins[3 * i + r] = o[r];
     dirs[3 * i + r] = d[r];
   }
-  area[i] = fmul(a.h_div, a.v_div);
-  times[i] = fadd(a.scan_time, dt);
+  area[i] = fmul(h_div, v_div);
+  times[i] = fadd(scan_time, dt);
+  if (a.sensor_idx) a.sensor_idx[i] = a.sweeps ? a.sweeps[s].sensor_idx : 0;
+  if (a.is_lidar) a.is_lidar[i] = 1;
+  if (a.index) {
+    a.index[3 * i] = s;
+    a.index[3 * i + 1] = b;
+    a.index[3 * i + 2] = k;
+  }
 }
 
 // ===================================================================================================== C ABI
@@ -2458,6 +2500,65 @@ int b200nerf_raygen_lidar_grid(b200nerf_ctx* c, const float* l2w_host, float ele
   if (velocity_host) memcpy(a.vel, velocity_host, sizeof(float) * 3);
   int64_t n = (int64_t)beams * n_azimuth;
   raygen_lidar_grid_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, origins, directions, pixel_area, times);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b200nerf_raygen_lidar_sweeps(b200nerf_ctx* c, const b200nerf_lidar_sweep* sweeps, int n_sweeps, int beams,
+                                 int n_azimuth, double azimuth_step_rad, const float* elevations,
+                                 const float* azimuth_offsets, float* origins, float* directions, float* pixel_area,
+                                 float* times, int64_t* sensor_idx, uint8_t* is_lidar, int* index, void* stream) {
+  REQUIRE(c && sweeps && elevations && origins && directions && pixel_area && times, "NULL argument");
+  REQUIRE(n_sweeps >= 1 && n_sweeps <= 65535, "n_sweeps must be in [1, 65535]");
+  REQUIRE(beams >= 1 && n_azimuth >= 1, "empty beam table or azimuth grid");
+  REQUIRE((int64_t)beams * n_azimuth * n_sweeps <= 0x7fffffff, "more than 2^31 - 1 rays");
+  REQUIRE(azimuth_step_rad > 0.0 && azimuth_step_rad < 1e300, "azimuth step must be finite and positive");
+  DeviceGuard g(c->device);
+  LidarGridArgs a{};
+  a.beams = beams; a.n_az = n_azimuth; a.az_step = azimuth_step_rad;
+  a.sweeps = sweeps; a.elev = elevations; a.az_off = azimuth_offsets;
+  a.sensor_idx = sensor_idx; a.is_lidar = is_lidar; a.index = index;
+  const int64_t per = (int64_t)beams * n_azimuth;
+  raygen_lidar_grid_kernel<<<dim3((unsigned)((per + 255) / 256), (unsigned)n_sweeps), 256, 0, (cudaStream_t)stream>>>(
+      a, origins, directions, pixel_area, times);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---- lidar simulation (lidar_sim.cuh)
+static int64_t lidar_sweep_tiles(int64_t rays_per_sweep) { return (rays_per_sweep + kLsTile - 1) / kLsTile; }
+
+size_t b200nerf_lidar_sweep_workspace_bytes(int n_sweeps, int64_t rays_per_sweep) {
+  if (n_sweeps < 1 || rays_per_sweep < 1) return 0;
+  return 2 * sizeof(int) * (size_t)n_sweeps * (size_t)lidar_sweep_tiles(rays_per_sweep);
+}
+
+int b200nerf_lidar_sweep_points(b200nerf_ctx* c, const b200nerf_lidar_sweep* sweeps, int n_sweeps, int beams,
+                                int n_azimuth, const float* origins, const float* directions, const float* times,
+                                const float* depth, const float* intensity, const float* ray_drop_prob, int use_ray_drop,
+                                float threshold, float* points_sensor, float* points_world, int* index, int* counts,
+                                int* offsets, void* workspace, size_t workspace_bytes, void* stream) {
+  REQUIRE(c, "ctx is NULL");
+  REQUIRE(n_sweeps >= 1 && n_sweeps <= 65535, "n_sweeps must be in [1, 65535]");
+  REQUIRE(beams >= 1 && n_azimuth >= 1, "empty beam table or azimuth grid");
+  const int64_t per = (int64_t)beams * n_azimuth;
+  REQUIRE(per * n_sweeps <= 0x7fffffff, "more than 2^31 - 1 rays");
+  REQUIRE(threshold - threshold == 0.0f, "threshold must be finite");
+  REQUIRE(sweeps && origins && directions && times && depth && intensity && points_sensor && points_world && index &&
+              counts && offsets && (ray_drop_prob || !use_ray_drop),
+          "NULL argument");
+  REQUIRE(workspace && workspace_bytes >= b200nerf_lidar_sweep_workspace_bytes(n_sweeps, per), "workspace too small");
+  DeviceGuard g(c->device);
+  const cudaStream_t s = (cudaStream_t)stream;
+  const int tiles = (int)lidar_sweep_tiles(per);
+  int* tile_counts = (int*)workspace;
+  int* tile_offsets = tile_counts + (int64_t)n_sweeps * tiles;
+  const LidarSweepArgs a{sweeps, per, n_azimuth, beams, tiles, origins, directions, times, depth, intensity,
+                         ray_drop_prob, use_ray_drop != 0, threshold};
+  const dim3 grid((unsigned)tiles, (unsigned)n_sweeps);
+  lidar_sweep_count_kernel<<<grid, kLsThreads, 0, s>>>(a, tile_counts);
+  lidar_sweep_scan_kernel<<<1, kLsScanThreads, 0, s>>>(n_sweeps, tiles, tile_counts, tile_offsets, counts, offsets);
+  lidar_sweep_emit_kernel<<<grid, kLsThreads, 0, s>>>(a, tile_offsets, points_sensor, points_world, index);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -91,6 +91,13 @@ class Camera(ctypes.Structure):
                 ("rolling_shutter_time", c_float), ("time_to_center_pixel", c_float), ("rs_direction", c_int32)]
 
 
+class LidarSweep(ctypes.Structure):
+    """b200nerf_lidar_sweep: one simulated sweep (nominal pose, time, rolling shutter, beam footprint, sensor index)."""
+
+    _fields_ = [("l2w", c_float * 12), ("scan_time", c_float), ("revolution_time", c_float), ("velocity", c_float * 3),
+                ("has_velocity", c_int32), ("h_div", c_float), ("v_div", c_float), ("sensor_idx", c_int32), ("pad_", c_int32)]
+
+
 SIGNATURES = {
     "b200nerf_last_error": (c_char_p, []),
     "b200nerf_version": (c_int, []),
@@ -186,6 +193,12 @@ SIGNATURES = {
     "b200nerf_raygen_lidar_points": (c_int, [c_void_p, POINTER(c_float), c_void_p, c_int, c_int64, c_float,
                                              POINTER(c_float), c_float, c_float, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_void_p, c_void_p]),
+    "b200nerf_raygen_lidar_sweeps": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200nerf_lidar_sweep_workspace_bytes": (c_size_t, [c_int, c_int64]),
+    "b200nerf_lidar_sweep_points": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
     "b200nerf_chamfer_distance": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int64, c_int, c_int, c_void_p,
                                           c_void_p, c_void_p, c_void_p]),
     "b200nerf_lidar_losses_workspace_bytes": (c_size_t, [c_int64]),

@@ -1627,6 +1627,71 @@ class NeuRADModel(nn.Module):
                 res["rgb_ready"] = done
         return res
 
+    @torch.no_grad()
+    def get_outputs_for_lidar_sweep(self, sensors, poses: Tensor, times, velocities: Optional[Tensor] = None,
+                                    ray_drop_threshold: Optional[float] = 0.5, max_distance: Optional[float] = None,
+                                    camera_indices=None) -> Dict[str, Tensor]:
+        """What a lidar would see from new poses: S simulated sweeps of scene.LidarSensor descriptors, the viewer's lidar
+        render (viewer/render_state_machine.py:391-430) generalised to beam tables, per-beam azimuth offsets, a rolling
+        shutter and several sweeps per call.
+
+        `sensors`: one LidarSensor or one per sweep, all with one beam count and azimuth resolution; poses [S,3,4]
+        sensor-to-world at the scan times; times [S]; velocities [S,3] or None.  The rays render as one 1-D lidar bundle
+        through `get_outputs_for_camera_ray_bundle`, in eval mode (the model's mode is restored afterwards), so actor
+        edits and, with use_camopt_in_eval, the camera optimizer act as on any render; `camera_indices` [S] names the
+        optimizer row of each sweep and is required when the optimizer applies.
+
+        A ray returns when ray_drop_prob < ray_drop_threshold if the threshold is not None and the model has a ray-drop
+        head (ray_drop_loss_mult > 0), else when depth < max_distance (None: non_return_lidar_distance); with the
+        defaults this is the rule of get_image_metrics_and_images (neurad.py:610-613).
+
+        Returns the render outputs over all N = S x beams x columns rays ([N,1] each), plus
+          depth_image / intensity_image / ray_drop_prob_image: [S, beams, columns] views of those outputs;
+          points [M,5]: the kept rays' origin + direction * depth in the frame of their sweep's nominal pose
+            (pose_inverse, models/ad_model.py:107-113) with intensity and the time offset from the scan time, the
+            layout of a measured scan (x, y, z, intensity, dt) -- `points[:, :3]` goes straight into chamfer_distance;
+          points_world [M,3]; point_index [M,3] int32 (sweep, beam, column), in that row-major order;
+          counts [S] and offsets [S] (int32, device): kept points per sweep and each sweep's first row.
+        The points are those of the generated rays, before any camera-optimizer correction, as in get_outputs_for_lidar.
+        Reading the kept count to size `points` is the call's one host synchronisation, given host (CPU) poses, times,
+        velocities, tables and camera_indices.  Each sensor_idx must lie in [0, config.num_sensors)."""
+        be = get_backend(self.static_scale.device)
+        for s_ in (sensors if isinstance(sensors, (list, tuple)) else [sensors]):
+            # the render indexes the appearance embedding with it unchecked
+            if not 0 <= int(s_.sensor_idx) < self.config.num_sensors:
+                raise ValueError(f"sensor_idx {s_.sensor_idx} is outside [0, {self.config.num_sensors}) (config.num_sensors)")
+        r = be.raygen_lidar_sweeps(sensors, poses, times, velocities)
+        n_sw, beams, n_az = r["shape"]
+        cam_idx = None
+        if camera_indices is not None:
+            ci = torch.as_tensor(camera_indices, dtype=torch.long).cpu().reshape(-1)
+            if ci.numel() != n_sw:
+                raise ValueError(f"camera_indices needs one entry per sweep ({n_sw}), got {ci.numel()}")
+            ci = ci.pin_memory().to(be.device, non_blocking=True)
+            cam_idx = ci[:, None].expand(n_sw, beams * n_az).reshape(-1, 1)
+        elif self.use_camopt_in_eval and self.camera_optimizer.config.mode != "off":
+            raise ValueError("the camera optimizer applies in eval (use_camopt_in_eval): pass camera_indices, one per sweep")
+        bundle = RayBundle(origins=r["origins"], directions=r["directions"], pixel_area=r["pixel_area"], times=r["times"],
+                           camera_indices=cam_idx, metadata={"is_lidar": r["is_lidar"], "sensor_idxs": r["sensor_idx"]})
+        was_training = self.training
+        self.eval()
+        try:
+            out = self.get_outputs_for_camera_ray_bundle(bundle)
+        finally:
+            self.train(was_training)
+        use_ray_drop = ray_drop_threshold is not None and self.config.ray_drop_loss_mult > 0.0
+        if use_ray_drop:
+            thr = float(ray_drop_threshold)
+        else:
+            thr = float(self.config.non_return_lidar_distance if max_distance is None else max_distance)
+        pts = be.lidar_sweep_points(r, out["depth"], out["intensity"], out["ray_drop_prob"] if use_ray_drop else None, thr)
+        m = int(pts["counts"][-1])
+        for k in ("depth", "intensity", "ray_drop_prob"):
+            out[f"{k}_image"] = out[k].view(n_sw, beams, n_az)
+        out["points"], out["points_world"], out["point_index"] = pts["points_sensor"][:m], pts["points_world"][:m], pts["index"][:m]
+        out["counts"], out["offsets"] = pts["counts"][:n_sw], pts["offsets"]
+        return out
+
     def set_decoder_stream(self, stream: Optional["torch.cuda.Stream"]) -> None:
         """Run the rgb decoder of `get_outputs_for_camera_ray_bundle` on a side stream (None: on the caller's stream, the
         default and the reference's behaviour).  With a stream, outputs["rgb"] must not be consumed before

@@ -225,6 +225,37 @@ class LidarScan:
     sensor_idx: int = 6
 
 
+@dataclass
+class LidarSensor:
+    """A spinning lidar for simulated sweeps (NeuRADModel.get_outputs_for_lidar_sweep): one ray per (beam, column).
+
+    Beam b points at elevation `elevations[b]` (radians, any order and spacing: the caller's beam table) and azimuth
+    column_azimuth + `azimuth_offsets[b]` (radians, None = 0).  The columns are the viewer's
+    `torch.arange(0, 2 pi, deg2rad(azimuth_resolution_deg))` (viewer/render_state_machine.py:396).  A ray's time offset
+    is that of its rotor column, (column_azimuth / 2 pi - 0.5) * revolution_time, and its origin moves with the sweep's
+    velocity over that offset (cameras/lidars.py:421-423, 625-639); revolution_time 0 puts every ray at the scan time.
+    pixel_area = h_div * v_div (the beam divergences of Lidars.generate_rays)."""
+
+    elevations: torch.Tensor  # [beams] radians
+    azimuth_resolution_deg: float
+    azimuth_offsets: Optional[torch.Tensor] = None  # [beams] radians
+    revolution_time: float = 0.1
+    h_div: float = 3.0e-3
+    v_div: float = 1.5e-3
+    sensor_idx: int = 6
+
+    @classmethod
+    def from_fov(cls, fov_min_deg: float, fov_max_deg: float, beams: int, azimuth_resolution_deg: float, **kw) -> "LidarSensor":
+        """Uniform elevations: the viewer's `torch.linspace(*np.deg2rad(lidar_fov), lidar_beams)`
+        (viewer/render_state_machine.py:395)."""
+        elev = torch.linspace(math.radians(fov_min_deg), math.radians(fov_max_deg), int(beams), dtype=torch.float32)
+        return cls(elevations=elev, azimuth_resolution_deg=azimuth_resolution_deg, **kw)
+
+    @property
+    def beams(self) -> int:
+        return int(torch.as_tensor(self.elevations).numel())
+
+
 def _look_at_c2w(pos: torch.Tensor, yaw: float, pitch: float = 0.0) -> torch.Tensor:
     """Camera-to-world for a camera at `pos` whose optical axis (-z) points along world yaw (about +z)."""
     fwd = torch.tensor([math.cos(yaw) * math.cos(pitch), math.sin(yaw) * math.cos(pitch), math.sin(pitch)])
