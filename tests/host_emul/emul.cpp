@@ -118,6 +118,14 @@ static const void* const* g_tcnn_ptrs = nullptr;
 static const int* g_tcnn_ints = nullptr;
 static const float* g_tcnn_floats = nullptr;
 static int g_bwd_generic = 0;  // 1: run the generic (MODE 0) scatter backward even where a fast path applies
+// actor edit of the following lane-mode renders (b200nerf_set_actor_edit): lateral, longitudinal, height, rotation, index
+static int g_edit_on = 0;
+static double g_edit[5];
+int emul_set_actor_edit(int on, const double* e) {
+  g_edit_on = on;
+  for (int i = 0; i < 5; ++i) g_edit[i] = on ? e[i] : 0.0;
+  return 0;
+}
 int emul_set_bwd_generic(int on) { g_bwd_generic = on; return 0; }
 int emul_set_tcnn(const void* const* ptrs, const int* ints, const float* floats) {
   g_tcnn_ptrs = ptrs; g_tcnn_ints = ints; g_tcnn_floats = floats;
@@ -194,6 +202,11 @@ int emul_render(const void* const* ptrs, const int* ints, const float* floats, l
       apply_tcnn(P, P.actors.n_actors);
       pol.sh_tcnn = 1;
       for (long long r = 0; r < n_rays; ++r) render_ray_lane<MlpLaneFfma, 1>(P, sc, pol, (int)(r % kLaneThreads), r, true);
+      return 0;
+    }
+    if (g_edit_on && !resolve_actor_edit(P.actors, g_edit[0], g_edit[1], g_edit[2], g_edit[3], g_edit[4])) return 2;
+    if (P.actors.edit_last > P.actors.edit_first) {
+      for (long long r = 0; r < n_rays; ++r) render_ray_lane<MlpLaneFfma, 0, true>(P, sc, pol, (int)(r % kLaneThreads), r, true);
       return 0;
     }
     for (long long r = 0; r < n_rays; ++r) render_ray_lane(P, sc, pol, (int)(r % kLaneThreads), r, true);

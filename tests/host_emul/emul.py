@@ -86,8 +86,10 @@ def _pack_params(pk, cfg, params, pdf_u, field_of_round):
     P(pdf_u(sp.num_nerf_samples))
     ints += list(field_of_round)
     P(params["appearance_embedding.weight"])
-    ints += [int(params["appearance_embedding.weight"].shape[0]), cfg.appearance_dim, cfg.embeds_per_sensor]
-    floats.append(cfg.duration)
+    # eps 0: one row per sensor, copied (use_temporal_appearance = False), as b200nerf_set_appearance_per_sensor sets it
+    eps = cfg.embeds_per_sensor if cfg.use_temporal_appearance else 0
+    ints += [int(params["appearance_embedding.weight"].shape[0]), cfg.appearance_dim, eps]
+    floats.append(cfg.duration if cfg.use_temporal_appearance else 1.0)
 
 
 def _tcnn_level_ints(layout):
@@ -120,9 +122,11 @@ def _torch_shaped_standin(cfg, params):
     return q
 
 
-def render(cfg, params, rays, pdf_u, field_of_round=(2, 2), lane_mode=False):
+def render(cfg, params, rays, pdf_u, field_of_round=(2, 2), lane_mode=False, edit=None):
     """cfg: neurad_studio_b200.NeuRADConfig; params: reference-named tensors (CPU); rays: dict of CPU tensors.  A
-    tcnn-layout parameter set (tcnn_compat.is_tcnn_state) runs the LAYOUT = 1 instantiation of the ray-per-lane code."""
+    tcnn-layout parameter set (tcnn_compat.is_tcnn_state) runs the LAYOUT = 1 instantiation of the ray-per-lane code.
+    `edit`: an actor_editing dict (lateral, longitudinal, height, rotation, index) resolved by resolve_actor_edit, as
+    b200nerf_set_actor_edit does (ray-per-lane mode, torch layout)."""
     from neurad_studio_b200 import tcnn_compat as T
 
     lib = ctypes.CDLL(build())
@@ -180,8 +184,14 @@ def render(cfg, params, rays, pdf_u, field_of_round=(2, 2), lane_mode=False):
         P(out[k])
         out[k] = keep[-1]
     c_ptrs, c_ints, c_floats = pk.c_arrays()
-    rc = lib.emul_render(c_ptrs, c_ints, c_floats, ctypes.c_longlong(n), ctypes.c_int(int(lane_mode)))
-    assert rc == 0
+    assert edit is None or lane_mode == 1, "actor edits are emulated in the ray-per-lane torch-layout code only"
+    e = (ctypes.c_double * 5)(*([float(edit[k]) for k in ("lateral", "longitudinal", "height", "rotation", "index")] if edit else [0.0] * 5))
+    lib.emul_set_actor_edit(ctypes.c_int(1 if edit else 0), e)
+    try:
+        rc = lib.emul_render(c_ptrs, c_ints, c_floats, ctypes.c_longlong(n), ctypes.c_int(int(lane_mode)))
+    finally:
+        lib.emul_set_actor_edit(ctypes.c_int(0), e)
+    assert rc == 0, rc
     del tcnn_keep
     return out
 

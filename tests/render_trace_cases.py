@@ -15,7 +15,7 @@ do not chain from stage to stage and no sample is compared against a sample plac
   3. the main field (sdf, field_feature) in float64 at the traced bins_e_2 with the last edge moved to the sky as the
      kernel does, the traced actor assignment (actor samples: 16 grid features padded to 32, the direction rotated into
      the box frame), and a per-entry bound carried through every MLP layer as gamma (|W| |a| + |b|) + |W| E_a: the
-     3xTF32 wgmma constant on the GPU (gamma_tc), the FFMA one in the emulation (gamma_ffma);
+     fp16 three-term split's constant on the GPU (gamma_f16), the FFMA one in the emulation (gamma_ffma);
   4. alpha from the traced sdf (bounded), weights from the traced alpha incl. the sky top-up (bit for bit);
   5. outputs: depth / accumulation / prop_depth_0 / _1 and the 16 appearance columns bit for bit (sequences of single
      IEEE roundings and double products the restatement repeats); features[:, :32] from the traced weights and field
@@ -54,24 +54,29 @@ class EmulRenderer:
     always records the full trace and has no lidar head: a partial trace only filters the returned fields, so the
     partial-trace comparisons are meaningful on the GPU only."""
 
-    def __init__(self, cfg, params):
-        self.cfg, self.params = cfg, params
+    def __init__(self, cfg, params, edit=None):
+        self.cfg, self.params, self.edit = cfg, params, edit
 
     def render(self, rays, want_trace=True, image_width=0, mode=None, want_intensity=False):
         from tests.host_emul import emul
 
-        out = emul.render(self.cfg, self.params, {k: v.cpu() for k, v in rays.items()}, O.pdf_u, lane_mode=True)
+        out = emul.render(self.cfg, self.params, {k: v.cpu() for k, v in rays.items()}, O.pdf_u, lane_mode=True,
+                          edit=self.edit)
         keep = set(TRACE_FIELDS) if want_trace is True else set(want_trace or ())
         return {k: v for k, v in out.items() if k not in TRACE_FIELDS or k in keep}
 
 
 class GpuRenderer:
-    def __init__(self, cfg, params):
+    """The library's render; an actor edit is set through the backend as NeuRADModel's eval render sets it."""
+
+    def __init__(self, cfg, params, edit=None):
         from neurad_studio_b200.backend import B200Backend
 
         self.cfg, self.params = cfg, params
         self.be = B200Backend(torch.device("cuda", 0))
         self.be.load_params(cfg, params)
+        if edit is not None:
+            self.be.set_actor_edit(**{k: edit[k] for k in EDIT_KEYS})
 
     def render(self, rays, want_trace=True, image_width=0, mode="split", want_intensity=False):
         from neurad_studio_b200.backend import DEFAULT_MODE
@@ -86,8 +91,8 @@ class GpuRenderer:
         return out
 
 
-def renderer(dev, cfg, params):
-    return EmulRenderer(cfg, params) if dev == "cpu" else GpuRenderer(cfg, params)
+def renderer(dev, cfg, params, edit=None):
+    return EmulRenderer(cfg, params, edit) if dev == "cpu" else GpuRenderer(cfg, params, edit)
 
 
 def _with_near_far(rays, seed):
@@ -111,15 +116,153 @@ def _cat(*bundles):
     return {k: torch.cat([b[k].cpu() for b in bundles]) for k in keys}
 
 
+EDIT_KEYS = ("lateral", "longitudinal", "height", "rotation", "index")
+# DynamicActors.actor_editing of the `edits` scene: a shift on all three box axes and a non-trivial yaw of one actor
+EDITS = {"edits": {"lateral": 0.6, "longitudinal": -1.1, "height": 0.15, "rotation": 0.7, "index": 1.0}}
+
+
+def scene_edit(name):
+    """The actor edit a scene renders under (None: unedited)."""
+    return EDITS.get(name)
+
+
+def edited_trajectories(trajs, edit):
+    """make_trajectories' dicts with the edit's selected actors at their edited poses (float64, for aiming rays)."""
+    out = [dict(t) for t in trajs]
+    c, s = np.cos(edit["rotation"]), np.sin(edit["rotation"])
+    yaw = torch.tensor([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]], dtype=torch.float64)
+    shift = torch.tensor([edit["lateral"], edit["longitudinal"], edit["height"]], dtype=torch.float64)
+    for a in edit_selection(len(trajs), edit):
+        p = trajs[a]["poses"].double().clone()
+        p[:, :3, 3] = p[:, :3, 3] + p[:, :3, :3] @ shift
+        p[:, :3, :3] = yaw @ p[:, :3, :3]
+        out[a]["poses"] = p.float()
+    return out
+
+
+def _sweep_scene(dev, table_scale):
+    """Viewer-style lidar sweeps (zero pixel area: every grid level at full weight) over four actors.  GPU: three sweeps
+    of a 32-beam LidarSensor.from_fov table at 1 degree columns from raygen_lidar_sweeps, at three poses and times with
+    rolling shutter and velocity, default tables.  CPU: the bundle and scene of tests/golden/lidar_sweep.npz (the
+    viewer's sweep; tables stored at 0.1 of the unit init) with the tables rescaled to `table_scale`."""
+    if dev == "cpu":
+        from tests import lidar_sim_cases as L
+
+        meta, cfg, params, g = L.golden()
+        k = table_scale / meta["table_scale"]
+        params = {key: (v * k if key.endswith("hash_table") else v) for key, v in params.items()}
+        n = g["ray"]["origins"].shape[0]
+        rays = {"origins": g["ray"]["origins"], "directions": g["ray"]["directions"], "pixel_area": torch.zeros(n, 1),
+                "times": torch.full((n, 1), float(meta["time"])),
+                "sensor_idx": torch.full((n, 1), meta["fallback_sensor_idx"], dtype=torch.long),
+                "is_lidar": torch.ones(n, 1, dtype=torch.bool)}
+        return cfg, params, rays, 0
+    from neurad_studio_b200.backend import B200Backend
+
+    cfg = nsb.NeuRADConfig(n_actors=4)
+    trajs = scene.make_trajectories(cfg.n_actors, cfg.duration, seed=21)
+    params = scene.make_params(cfg, seed=21, table_scale=table_scale, beta=4.0, sdf_bias=0.5, trajectories=trajs)
+    sensor = scene.LidarSensor.from_fov(-25.0, 15.0, 32, 1.0, h_div=0.0, v_div=0.0)
+    poses = torch.zeros(3, 3, 4)
+    poses[:, :, :3] = torch.eye(3)
+    poses[:, :, 3] = torch.tensor([[10.0, 0.0, 1.8], [22.0, 0.5, 1.8], [33.0, -0.5, 1.9]])
+    be = B200Backend(torch.device("cuda", 0))
+    sw = be.raygen_lidar_sweeps(sensor, poses, [1.0, 2.0, 3.0], velocities=[[10.0, 0.0, 0.0]] * 3)
+    n = sw["origins"].shape[0]
+    rays = {k: sw[k].cpu().reshape(n, -1) for k in ("origins", "directions", "pixel_area", "times", "sensor_idx", "is_lidar")}
+    assert (rays["pixel_area"] == 0).all() and rays["is_lidar"].all()
+    return cfg, params, rays, 0
+
+
+# Depth tolerance (of the maximum) of a zero-area sweep over unit-scale tables against the reference.  The reference's
+# own arithmetic moves by 3.6e-4 there when only its exp() is rounded differently (sweep_oracle(exact_exp=True): SLEEF's
+# vectorised exp against a correctly rounded one), while every stage of the kernels stays inside its per-entry bound
+# (the sweep_unit trace).  The library, which differs from the reference in its exp and its sum orders too, is 3.9e-4
+# away (H100); the host emulation of the same device code 2.6e-4.  5e-4 is that floor with the margin of a second
+# independent rounding of the same size.
+SWEEP_UNIT_DEPTH_TOL = 5e-4
+
+
+def sweep_golden_scene(table_scale):
+    """(cfg, params, rays) of the lidar-sweep golden's scene with its tables at `table_scale` of the unit init."""
+    cfg, params, rays, _ = _sweep_scene("cpu", table_scale)
+    return cfg, params, rays
+
+
+def sweep_oracle(table_scale, exact_exp=False):
+    """The reference's math (the oracle) on sweep_golden_scene(table_scale); `exact_exp`: torch.exp of fp32 tensors
+    rounded correctly (computed in double) instead of torch's vectorised SLEEF routine, the one change
+    tests/test_reference_noise_floor.py makes."""
+    from oracle.convert import to_oracle_cfg
+
+    cfg, params, r = sweep_golden_scene(table_scale)
+    orig = torch.exp
+    if exact_exp:
+        torch.exp = lambda x, *a, **k: orig(x.double()).float() if x.dtype == torch.float32 else orig(x, *a, **k)
+    try:
+        with torch.no_grad():
+            return O.nff_outputs(params, to_oracle_cfg(cfg), r["origins"], r["directions"], r["pixel_area"], r["times"],
+                                 r["sensor_idx"], r["is_lidar"])
+    finally:
+        torch.exp = orig
+
+
+def rel_to_max(a, b):
+    a, b = a.detach().cpu().double(), b.detach().cpu().double()
+    return (a.reshape(b.shape) - b).abs().max().item() / (b.abs().max().item() + 1e-30)
+
+
+def _small_tables(cfg, log2_main=12, log2_prop=11):
+    """cfg with small_config's table sizes (levels and resolutions kept)."""
+    cfg.grid.static.log2_hashmap_size = log2_main
+    cfg.grid.actor.log2_hashmap_size = max(log2_main - 3, 6)
+    for g in cfg.proposal_grids:
+        g.static.log2_hashmap_size = log2_prop
+        g.actor.log2_hashmap_size = max(log2_prop - 3, 6)
+    return cfg
+
+
 def scene_rays(dev, name):
-    """(cfg, params, rays, image_width) of one test scene.
+    """(cfg, params, rays, image_width) of one test scene (scene_edit(name): its actor edit).
 
     config2: NeuRADConfig(n_actors=0), default tables on the GPU; one PandaSet camera at render stride 3 (640 x 360, the
       2-D tile walk has ragged 16-row tiles at the bottom) followed by a lidar sweep (is_lidar: area scale 1), with
       nears / fars on every ray, some fars below the sky distance.
     config3: 16 actors, rays aimed at the boxes, a ray count that is not a multiple of 32, 128 or 512.
-    opaque: a dense proposal field, so that the proposal transmittance underflows within a few samples in whole warps."""
+    opaque: a dense proposal field, so that the proposal transmittance underflows within a few samples in whole warps.
+    sweep_unit / sweep_tenth: zero-area lidar sweeps over four actors (_sweep_scene), unit tables and 0.1 of them.
+    init_scale: tables at the reference's hash_init_scale 1e-3 (field_components/encodings.py:333).
+    f16_small: tables at 1e-4 and every MLP bias 0: small activations, where the fp16 split's lo parts are subnormal.
+    edits: config3 with the actor edit EDITS["edits"].
+    paper / neurader: nsb.preset(...) (one appearance row per sensor; doubled static resolutions, finest main level
+      16383 cells, 2^23-row main table at production size on the GPU; small tables on the CPU)."""
     gpu = dev != "cpu"
+    if name in ("sweep_unit", "sweep_tenth"):
+        return _sweep_scene(dev, 1.0 if name == "sweep_unit" else 0.1)
+    if name in ("init_scale", "f16_small"):
+        cfg = nsb.NeuRADConfig(n_actors=0) if gpu else nsb.small_config()
+        params = scene.make_params(cfg, seed=71, table_scale=1e-3 if name == "init_scale" else 1e-4, beta=4.0)
+        if name == "f16_small":
+            for k in params:
+                if k.startswith("field.mlp_") and k.endswith(".bias"):
+                    params[k] = torch.zeros_like(params[k])
+        rays = scene.random_rays(4100 if gpu else 160, cfg, seed=72)
+        return cfg, params, rays, 0
+    if name == "edits":  # config3's scene, half the rays aimed at the boxes at their edited poses, half of those at the edited actor
+        cfg = nsb.NeuRADConfig(n_actors=16) if gpu else nsb.small_config(n_actors=16)
+        trajs = scene.make_trajectories(cfg.n_actors, cfg.duration, seed=21)
+        params = scene.make_params(cfg, seed=21, beta=4.0, sdf_bias=0.5, trajectories=trajs)
+        aim = edited_trajectories(trajs, EDITS[name])
+        aim = aim + [aim[a] for a in edit_selection(cfg.n_actors, EDITS[name])] * cfg.n_actors
+        rays = scene.random_rays(8227 if gpu else 1201, cfg, seed=22, trajectories=aim)
+        return cfg, params, rays, 0
+    if name in ("paper", "neurader"):
+        cfg, _ = nsb.preset("neurad-paper" if name == "paper" else "neurader")
+        if not gpu:
+            cfg = _small_tables(cfg)
+        params = scene.make_params(cfg, seed=81, beta=4.0, sdf_bias=0.5)
+        rays = scene.random_rays(8200 if gpu else 200, cfg, seed=82)
+        return cfg, params, _with_near_far(rays, 83), 0
     if name == "config2":
         cfg = nsb.NeuRADConfig(n_actors=0) if gpu else nsb.small_config()
         params = scene.make_params(cfg, seed=41, beta=3.0, sdf_bias=0.6)
@@ -239,8 +382,12 @@ def merge_walk(w, edges_s, u, hist_pad):
 
 
 def appearance_bits(cfg, params, times, sensor):
-    """The temporal appearance columns, op by op as the kernel evaluates them (fp32, single roundings)."""
+    """The appearance columns, op by op as the kernel evaluates them (fp32, single roundings): with
+    use_temporal_appearance the sensor's two rows around the time, interpolated; without it (the paper presets) the row
+    `sensor`, copied (neurad.py:440)."""
     emb = params["appearance_embedding.weight"].float().cpu()
+    if not cfg.use_temporal_appearance:
+        return emb[sensor.long().reshape(-1)]
     eps_ = _f(float(cfg.embeds_per_sensor))
     tidx = (times.float() / _f(cfg.duration)) * eps_
     before = torch.clamp(torch.clamp_min(torch.floor(tidx), 0.0), max=eps_ - 1.0)
@@ -436,12 +583,49 @@ def _dot3(a, b):
     return (a[..., 0] * b[..., 0] + a[..., 1] * b[..., 1]) + a[..., 2] * b[..., 2]
 
 
+def edit_selection(n_actors, edit):
+    """The actors an actor edit moves, by the reference's own indexing (tests/actor_edit_cases.py); [] for no edit."""
+    from tests.actor_edit_cases import torch_selection
+
+    sel = None if edit is None else torch_selection(n_actors, edit)
+    return [] if sel is None else sel
+
+
+def edit_cos_sin(edit):
+    """cos / sin of the edit's yaw taken in double and rounded once to fp32, as resolve_actor_edit does."""
+    r = float(edit["rotation"])
+    return float(np.float32(np.cos(r))), float(np.float32(np.sin(r)))
+
+
+def _edit_pose32(b1, b2, b3, pos, edit, corrupt=None):
+    """edit_box_pose in fp32, op by op, on the rows b1, b2, b3 [n, A, 3] of box -> world and the centre pos [n, A, 3]:
+    pos' = R shift + pos (box-frame shift, unedited R), then rows (c b1 - s b2, s b1 + c b2, b3).  `corrupt`:
+    "world_shift" adds the shift in the world frame (the self-tests)."""
+    sel = edit_selection(b1.shape[1], edit)
+    if not sel:
+        return b1, b2, pos
+    s = _f([edit["lateral"], edit["longitudinal"], edit["height"]])
+    c, sn = (_f(v) for v in edit_cos_sin(edit))
+    m = torch.zeros(b1.shape[1], dtype=torch.bool)
+    m[sel] = True
+    m = m[None, :, None]
+    if corrupt == "world_shift":
+        new_pos = pos + s
+    else:
+        new_pos = torch.stack([((b[..., 0] * s[0] + b[..., 1] * s[1]) + b[..., 2] * s[2]) + pos[..., i]
+                               for i, b in enumerate((b1, b2, b3))], -1)
+    nb1, nb2 = c * b1 - sn * b2, sn * b1 + c * b2
+    return torch.where(m, nb1, b1), torch.where(m, nb2, b2), torch.where(m, new_pos, pos)
+
+
 class ActorFrames:
     """The per-ray actor frames of lane_actor_candidates (after the keyframe Gram-Schmidt of actors_prep_kernel), op by
     op in fp32 on the CPU: rotation R [n, A, 3, 3] and translation t [n, A, 3] of world -> box, the padded half sizes
-    [A, 3], validity and the ray-line cull.  box() gives the kernel's box-frame position of a sample bit for bit."""
+    [A, 3], validity and the ray-line cull.  box() gives the kernel's box-frame position of a sample bit for bit.
+    `edit`: the actor edit the render ran under (edit_box_pose, applied after the Gram-Schmidt); `corrupt` as in
+    _edit_pose32."""
 
-    def __init__(self, params, cfg, o, d, times):
+    def __init__(self, params, cfg, o, d, times, edit=None, corrupt=None):
         rot6 = params["dynamic_actors.actor_rotations_6d"].detach().float().cpu()
         pos = params["dynamic_actors.actor_positions"].detach().float().cpu()
         ts = params["dynamic_actors.unique_timestamps"].detach().float().cpu()
@@ -462,9 +646,10 @@ class ActorFrames:
         b2 = _normalize3(p[..., 3:6] - _dot3(b1, p[..., 3:6])[..., None] * b1)
         b3 = torch.stack([b1[..., 1] * b2[..., 2] - b1[..., 2] * b2[..., 1], b1[..., 2] * b2[..., 0] - b1[..., 0] * b2[..., 2],
                           b1[..., 0] * b2[..., 1] - b1[..., 1] * b2[..., 0]], -1)
+        b1, b2, pos = _edit_pose32(b1, b2, b3, p[..., 6:9], edit, corrupt)
         self.R = torch.stack([b1, b2, b3], -1)  # R[..., i, j] = b_j[i]: row i of world -> box
-        self.t = -_dot3(self.R, p[..., None, 6:9])
-        self.pos = p[..., 6:9]
+        self.t = -_dot3(self.R, pos[..., None, :])
+        self.pos = pos
         pad = params.get("dynamic_actors.actor_padding")
         pad = torch.tensor(list(cfg.actor_bbox_padding)) if pad is None else pad.detach().float().cpu()
         self.bounds = params["dynamic_actors.actor_sizes"].detach().float().cpu() * 0.5 + pad.float()
@@ -495,8 +680,16 @@ def _grid(tables, F, T, scalings, c32, cs64, dev, base=None):
         f56, f47 = c[5] * ox + c[6] * (1 - ox), c[4] * ox + c[7] * (1 - ox)
         return (f03 * oy + f12 * (1 - oy)) * oz + (f47 * oy + f56 * (1 - oy)) * (1 - oz)
 
-    t = sc.to(dev).double()[None, :] * 2 * cs64.to(dev)[:, None]
-    return tri(f), tri(f.abs()), 1.0 / t.clamp_min(1.0), t
+    lw, t = level_weights64(sc, cs64.to(dev))
+    return tri(f), tri(f.abs()), lw, t
+
+
+def level_weights64(scalings, cs64):
+    """float64 level weights 1 / max(1, 2 res std) [P, L] and their argument t, at the contracted std cs64 [P].  Zero
+    pixel area (a viewer / simulated lidar sweep) gives std 0, t 0 and lw == 1 exactly: every level at full weight,
+    and _level_terms carries no level-weight error there."""
+    t = scalings.to(cs64.device).double()[None, :] * 2 * cs64[:, None]
+    return 1.0 / t.clamp_min(1.0), t
 
 
 def _level_terms(v, vabs, lw, t):
@@ -519,6 +712,8 @@ class FieldSamples:
         self.n, self.S = e.shape[0], e.shape[1] - 1
         g32 = _gauss32(o.float(), d.float(), area.float(), e.float())
         self.mean64, std64 = _gauss64(o, d, area, e)
+        zero = (area.reshape(-1) == 0)[:, None].expand(self.n, self.S)
+        assert (std64[zero] == 0).all(), "zero pixel area must give std 0 (every level at full weight)"
         self.aid = aid.reshape(-1).long()
         self.static = self.aid < 0
         scale = float(params["static_scale"])
@@ -601,8 +796,8 @@ def _ray_inputs(rays, idx, cfg):
     return o, d, area, rays["times"].reshape(-1)[idx].float()
 
 
-def _frames(params, cfg, o, d, times):
-    return ActorFrames(params, cfg, o, d, times) if cfg.n_actors else None
+def _frames(params, cfg, o, d, times, edit=None):
+    return ActorFrames(params, cfg, o, d, times, edit) if cfg.n_actors else None
 
 
 def round0_edges(cfg, rays, idx):
@@ -620,9 +815,9 @@ def main_edges(cfg, bins_e_2):
     return e
 
 
-def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048):
-    """Stage 1 on every ray (actor samples through the actor's proposal grid, at the kernel's fp32 box positions);
-    returns (worst ratio, excl lower bounds of round 0 [n, S0])."""
+def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048, edit=None):
+    """Stage 1 on every ray (actor samples through the actor's proposal grid, at the kernel's fp32 box positions, under
+    the actor edit `edit`); returns (worst ratio, excl lower bounds of round 0 [n, S0])."""
     o, d, area, times = _ray_inputs(rays, idx, cfg)
     e0 = round0_edges(cfg, rays, idx)
     worst, low0 = 0.0, None
@@ -631,8 +826,8 @@ def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048):
         w_all, tol_all, low_all = [], [], []
         for c0 in range(0, idx.numel(), chunk):
             c = slice(c0, c0 + chunk)
-            fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c]), o[c], d[c], area[c], times[c], e[c],
-                              aid[c], cfg.proposal_grid_2.actor_scale)
+            fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c], edit), o[c], d[c], area[c], times[c],
+                              e[c], aid[c], cfg.proposal_grid_2.actor_scale)
             dens, rel = proposal_density_reference(params, cfg, fs, dev)
             w, tol, low = proposal_weights_reference(dens, rel, e[c])
             w_all.append(w), tol_all.append(tol), low_all.append(low)
@@ -650,6 +845,14 @@ def gamma_tc(K):
     products and the bias are accumulated in fp32 in an unspecified order and rounding mode (truncation allowed): each of
     the 3 K + 1 additions <= 2^-22 of the running sum, <= 2^-22 (3 K + 1) of sum |terms|."""
     return 3 * 2.0 ** -20 + (3 * K + 1) * 2.0 ** -22
+
+
+def gamma_f16(K):
+    """Per-term constant of one fp16 three-term layer with K inputs (MlpLaneTc, the lane kernels' MLP; DESIGN section 4):
+    the split's representation and dropped lo * lo terms, <= 3.0001 2^-22 |a w| (rounded up to 4 2^-22, which also
+    covers the subnormal absolute term of the lo parts for activations down to 1e-4, tests/test_zz_f16_mlp_gpu.py), plus
+    the same fp32 accumulation term as gamma_tc, (3 K + 1) 2^-22."""
+    return 4 * 2.0 ** -22 + (3 * K + 1) * 2.0 ** -22
 
 
 def gamma_ffma(K):
@@ -746,17 +949,17 @@ def main_field_reference(params, cfg, fs, d, dev, gamma, corrupt=None):
     return sdf.reshape(n, S).cpu(), E_sdf.reshape(n, S).cpu(), feat.reshape(n, S, 32).cpu(), E_feat.reshape(n, S, 32).cpu()
 
 
-def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048):
+def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048, edit=None):
     """Stage 3: sdf and field_feature of every sample against main_field_reference at the traced bins_e_2 (the last edge
-    moved to the sky), with the traced actor assignment.  Returns the worst ratios."""
+    moved to the sky), with the traced actor assignment under the actor edit `edit`.  Returns the worst ratios."""
     o, d, area, times = _ray_inputs(rays, idx, cfg)
     e = main_edges(cfg, tr["bins_e_2"])
     aid = tr.get("actor_id_main", torch.full(e[:, 1:].shape, -1, dtype=torch.int32))
     ws, wf = 0.0, 0.0
     for c0 in range(0, idx.numel(), chunk):
         c = slice(c0, c0 + chunk)
-        fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c]), o[c], d[c], area[c], times[c], e[c], aid[c],
-                          cfg.grid.actor_scale)
+        fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c], edit), o[c], d[c], area[c], times[c], e[c],
+                          aid[c], cfg.grid.actor_scale)
         sdf, Es, feat, Ef = main_field_reference(params, cfg, fs, d[c], dev, gamma)
         ws = max(ws, _ratio(tr["sdf"][c], sdf, Es, "sdf"))
         wf = max(wf, _ratio(tr["field_feature"][c], feat, Ef, "field_feature"))
@@ -764,15 +967,34 @@ def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048):
 
 
 # ====================================================================================== stage 6: actor ids
-def check_actor_ids(tr, rays, idx, cfg, params, chunk=512):
+def edit_boxes2world64(b2w, edit, corrupt=None):
+    """DynamicActors.edit_boxes2world (oracle/actor_edit_oracle.py) in float64 on b2w [n, A, 3|4, 4], with the kernel's
+    fp32 shift and its cos / sin rounded once (edit_cos_sin): t' = R shift + t, R' = Rz(yaw) R.  `corrupt` as in
+    _edit_pose32."""
+    sel = edit_selection(b2w.shape[1], edit)
+    if not sel:
+        return b2w
+    b2w = b2w.clone()
+    shift = torch.tensor([float(np.float32(edit[k])) for k in ("lateral", "longitudinal", "height")], dtype=torch.float64)
+    R = b2w[:, sel, :3, :3]
+    b2w[:, sel, :3, 3] = b2w[:, sel, :3, 3] + (shift if corrupt == "world_shift" else R @ shift)
+    c, s = edit_cos_sin(edit)
+    yaw = torch.tensor([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]], dtype=torch.float64)
+    b2w[:, sel, :3, :3] = yaw @ R
+    return b2w
+
+
+def check_actor_ids(tr, rays, idx, cfg, params, chunk=512, edit=None, corrupt=None):
     """actor_id_0 / _1 / _main against a float64 box test of the float64 sample means at the traced edges: the highest
     actor whose padded box (the fp32 half sizes) strictly contains the mean, among the actors present at a bracketing
-    keyframe.  A mismatch is allowed only where the float64 box coordinate of some present actor lies within
-    64 U (|mean| + |box centre| + half size) of a face (the kernel's fp32 frame is a few ulp of those magnitudes off).
+    keyframe, at the poses the actor edit `edit` gives (edit_boxes2world64; `corrupt` for the self-tests).  A mismatch
+    is allowed only where the float64 box coordinate of some present actor lies within 64 U (|mean| + |box centre| +
+    half size) of a face (the kernel's fp32 frame is a few ulp of those magnitudes off).
     Returns (mismatches at a face, samples compared)."""
     o, d, area, times = _ray_inputs(rays, idx, cfg)
     p64 = {k: (v.double() if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in params.items()}
     b2w, valid = O.boxes2world_at(p64, times.double())
+    b2w = edit_boxes2world64(b2w, edit, corrupt)
     w2b = O.pose_inverse(b2w)  # [n, A, 3, 4]
     fr = ActorFrames(params, cfg, o, d, times)
     bnd = fr.bounds.double()
@@ -839,13 +1061,18 @@ def select(out, idx):
     return {k: v[idx.to(v.device)].cpu() for k, v in out.items()}
 
 
-def check_scene(dev, name, mode="split", n_random=127, report=print):
+def check_scene(dev, name, mode="split", n_random=127, report=print, gamma=None):
     """Full trace of one scene: every stage on whole 128-ray warp groups (every ray on the CPU); then a render with a
     partial trace (no actor ids: the early exit on) and an untraced render must match the full trace bit for bit.
+    `gamma`: the MLP's per-term constant of the main-field bounds; by default the one of the MLP that ran, gamma_ffma
+    in the emulation and gamma_f16 for the lane kernels' fp16 split on the GPU.
     Returns (worst ratio per stage, inferred early-exit warps, actor-id face exceptions, full render, referenced rays)."""
     t0 = time.perf_counter()
+    if gamma is None:
+        gamma = gamma_ffma if dev == "cpu" else gamma_f16
     cfg, params, rays, width = scene_rays(dev, name)
-    r = renderer(dev, cfg, params)
+    edit = scene_edit(name)
+    r = renderer(dev, cfg, params, edit)
     rd = {k: (v.to(dev) if dev != "cpu" else v) for k, v in rays.items()}
     full = r.render(rd, want_trace=True, image_width=width, mode=mode, want_intensity=True)
     n = rays["origins"].shape[0]
@@ -859,16 +1086,21 @@ def check_scene(dev, name, mode="split", n_random=127, report=print):
     check_walk(out, rays, idx, cfg)
     worst.update(check_shading(out, out, rays, idx, cfg, params))
     fdev = "cpu" if dev == "cpu" else dev
-    worst["prop_weights"], low = check_proposal_weights(out, rays, idx, cfg, params, fdev)
-    worst.update(check_main_field(out, rays, idx, cfg, params, fdev, gamma_ffma if dev == "cpu" else gamma_tc))
+    worst["prop_weights"], low = check_proposal_weights(out, rays, idx, cfg, params, fdev, edit=edit)
+    worst.update(check_main_field(out, rays, idx, cfg, params, fdev, gamma, edit=edit))
     if "intensity" in out:
         worst.update(check_lidar(out, cfg, params))
     exits = early_exit_warps(low, idx) if width == 0 else 0
     faces = 0
     if cfg.n_actors:
         hits = int((out["actor_id_main"] >= 0).sum())
-        assert hits >= max(10, n // 40), f"{name}: only {hits} actor samples: the actor branch is not exercised"
-        faces, _ = check_actor_ids(out, rays, idx, cfg, params)
+        # sweeps are not aimed at the boxes: the GPU's three 32-beam sweeps put ~600 samples in them, the golden's viewer
+        # sweep (8 beams, 7.5 degree columns) a handful
+        need = max(10, n // 40) if not name.startswith("sweep") else 0 if dev == "cpu" else 300
+        assert hits >= need, f"{name}: only {hits} actor samples: the actor branch is not exercised"
+        faces, _ = check_actor_ids(out, rays, idx, cfg, params, edit=edit)
+        for a in edit_selection(cfg.n_actors, edit):
+            assert int((out["actor_id_main"] == a).sum()) >= 10, f"{name}: edited actor {a} is hardly hit"
     # the traced fields and outputs do not depend on what else is traced (on the CPU the emulation always traces
     # everything, so these comparisons only bite on the GPU)
     part = r.render(rd, want_trace=PARTIAL, image_width=width, mode=mode)

@@ -4,7 +4,8 @@ power-of-two scaled operands, fp32 accumulation.
   * on the GPU, the traced sdf and field features of both lane kernels stay inside the per-entry float64 bounds of
     tests/render_trace_cases.py with the fp16 split's own constant gamma_f16, which is tighter than gamma_tc;
   * on the CPU, a float64 emulation of the scaled split shows that the three-term split meets gamma_f16 and that a
-    two-term split (without a_hi * w_lo) does not;
+    two-term split (without a_hi * w_lo) does not, and where gamma_f16 stops holding as activations shrink (down to
+    1e-4 it holds, at 1e-5 the subnormal lo parts break it);
   * on the GPU, parameters that push an activation beyond the fp16 operand range raise the device status instead of
     rendering inf or NaN."""
 import pytest
@@ -17,11 +18,7 @@ from tests import render_trace_cases as C
 A_EXP = 6  # kLaneTcA: A operands are 2^6 times the activations
 
 
-def gamma_f16(K):
-    """Per-term constant of one fp16 three-term layer with K inputs (DESIGN section 4): the split's representation
-    and dropped lo * lo terms, <= 3.0001 2^-22 |a w| (rounded up to 4 2^-22, which also covers the subnormal absolute
-    term at the kernel's scales), plus the same fp32 accumulation term as gamma_tc, (3 K + 1) 2^-22."""
-    return 4 * 2.0 ** -22 + (3 * K + 1) * 2.0 ** -22
+gamma_f16 = C.gamma_f16
 
 
 def test_gamma_f16_is_tighter_than_gamma_tc():
@@ -63,6 +60,26 @@ def test_split_emulation_meets_gamma_f16_and_two_terms_do_not(K):
     except AssertionError:
         return
     raise AssertionError("gamma_f16 accepted a two-term split")
+
+
+@pytest.mark.parametrize("scale", [1.0, 1e-3, 1e-4, 1e-5])
+def test_split_emulation_meets_gamma_f16_down_to_activations_of_1e4(scale):
+    """Where gamma_f16 stops holding.  Bias-free layers with K = 32 nn.Linear-sized weights and activations uniform in
+    [-scale, scale]: once the scaled activations' lo parts are fp16 subnormals, their absolute rounding (half the
+    subnormal spacing) is not proportional to |a w|.  The bound holds down to activations of 1e-4 (the reference's
+    hash_init_scale is 1e-3) and fails at 1e-5."""
+    gen = torch.Generator().manual_seed(0)
+    K = 32
+    a = (torch.rand(4096, K, generator=gen) * 2 - 1).float() * scale
+    w = ((torch.rand(32, K, generator=gen) * 2 - 1) / K ** 0.5).float()
+    ref = a.double() @ w.double().T
+    tol = gamma_f16(K) * (a.double().abs() @ w.double().abs().T)
+    worst = ((_layer(a, w, 3) - ref).abs() / tol).max().item()
+    print(f"\n[f16 mlp] activations ~{scale:g}: worst |err| / gamma_f16 bound {worst:.3g}")
+    if scale >= 1e-4:
+        assert worst < 0.5, worst
+    else:
+        assert worst > 1.0, f"gamma_f16 now holds at activations of {scale:g} ({worst:.3g}): update DESIGN section 4"
 
 
 @pytest.mark.gpu
