@@ -198,13 +198,17 @@ int emul_render(const void* const* ptrs, const int* ints, const float* floats, l
     LaneScratch sc = lane_scratch_of(scratch.data(), 0);
     std::vector<float> panel((size_t)kNff * kLaneThreads);
     MlpLaneFfma pol{mlp.data(), panel.data()};
+    if (g_edit_on && !resolve_actor_edit(P.actors, g_edit[0], g_edit[1], g_edit[2], g_edit[3], g_edit[4])) return 2;
     if (lane_mode == 2) {
       apply_tcnn(P, P.actors.n_actors);
       pol.sh_tcnn = 1;
+      if (P.actors.edit_last > P.actors.edit_first) {
+        for (long long r = 0; r < n_rays; ++r) render_ray_lane<MlpLaneFfma, 1, true>(P, sc, pol, (int)(r % kLaneThreads), r, true);
+        return 0;
+      }
       for (long long r = 0; r < n_rays; ++r) render_ray_lane<MlpLaneFfma, 1>(P, sc, pol, (int)(r % kLaneThreads), r, true);
       return 0;
     }
-    if (g_edit_on && !resolve_actor_edit(P.actors, g_edit[0], g_edit[1], g_edit[2], g_edit[3], g_edit[4])) return 2;
     if (P.actors.edit_last > P.actors.edit_first) {
       for (long long r = 0; r < n_rays; ++r) render_ray_lane<MlpLaneFfma, 0, true>(P, sc, pol, (int)(r % kLaneThreads), r, true);
       return 0;

@@ -126,7 +126,7 @@ def render(cfg, params, rays, pdf_u, field_of_round=(2, 2), lane_mode=False, edi
     """cfg: neurad_studio_b200.NeuRADConfig; params: reference-named tensors (CPU); rays: dict of CPU tensors.  A
     tcnn-layout parameter set (tcnn_compat.is_tcnn_state) runs the LAYOUT = 1 instantiation of the ray-per-lane code.
     `edit`: an actor_editing dict (lateral, longitudinal, height, rotation, index) resolved by resolve_actor_edit, as
-    b200nerf_set_actor_edit does (ray-per-lane mode, torch layout)."""
+    b200nerf_set_actor_edit does (ray-per-lane mode, either layout)."""
     from neurad_studio_b200 import tcnn_compat as T
 
     lib = ctypes.CDLL(build())
@@ -184,7 +184,7 @@ def render(cfg, params, rays, pdf_u, field_of_round=(2, 2), lane_mode=False, edi
         P(out[k])
         out[k] = keep[-1]
     c_ptrs, c_ints, c_floats = pk.c_arrays()
-    assert edit is None or lane_mode == 1, "actor edits are emulated in the ray-per-lane torch-layout code only"
+    assert edit is None or lane_mode in (1, 2), "actor edits are emulated in the ray-per-lane code only"
     e = (ctypes.c_double * 5)(*([float(edit[k]) for k in ("lateral", "longitudinal", "height", "rotation", "index")] if edit else [0.0] * 5))
     lib.emul_set_actor_edit(ctypes.c_int(1 if edit else 0), e)
     try:

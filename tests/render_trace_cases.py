@@ -222,6 +222,24 @@ def _small_tables(cfg, log2_main=12, log2_prop=11):
     return cfg
 
 
+def camera_and_lidar_rays(cfg):
+    """One PandaSet camera through the GPU's ray generation at render stride 3 (640 x 360, the 2-D tile walk has ragged
+    16-row tiles at the bottom) followed by a lidar sweep (is_lidar: area scale 1); returns (CPU rays, image width)."""
+    from neurad_studio_b200.backend import B200Backend
+
+    be = B200Backend(torch.device("cuda", 0))
+    cam = be.raygen_pinhole(scene.pandaset_rig()[0], row0=1, row_step=3, col0=1, col_step=3)
+    lid = be.raygen_lidar_points(scene.pandar64_scan())
+    n_cam, n_lid, width = cam["origins"].shape[0], lid["origins"].shape[0] - 77, 640
+    keys = ("origins", "directions", "pixel_area", "times")
+    cam = {k: cam[k].cpu().reshape(n_cam, -1) for k in keys}
+    lid = {k: lid[k].cpu().reshape(-1, cam[k].shape[1])[:n_lid] for k in keys}
+    cam["is_lidar"], lid["is_lidar"] = torch.zeros(n_cam, 1, dtype=torch.bool), torch.ones(n_lid, 1, dtype=torch.bool)
+    cam["sensor_idx"] = torch.zeros(n_cam, 1, dtype=torch.long)
+    lid["sensor_idx"] = torch.full((n_lid, 1), cfg.num_sensors - 1, dtype=torch.long)
+    return _cat(cam, lid), width
+
+
 def scene_rays(dev, name):
     """(cfg, params, rays, image_width) of one test scene (scene_edit(name): its actor edit).
 
@@ -267,19 +285,7 @@ def scene_rays(dev, name):
         cfg = nsb.NeuRADConfig(n_actors=0) if gpu else nsb.small_config()
         params = scene.make_params(cfg, seed=41, beta=3.0, sdf_bias=0.6)
         if gpu:
-            from neurad_studio_b200.backend import B200Backend
-
-            be = B200Backend(torch.device("cuda", 0))
-            cam = be.raygen_pinhole(scene.pandaset_rig()[0], row0=1, row_step=3, col0=1, col_step=3)
-            lid = be.raygen_lidar_points(scene.pandar64_scan())
-            n_cam, n_lid, width = cam["origins"].shape[0], lid["origins"].shape[0] - 77, 640
-            keys = ("origins", "directions", "pixel_area", "times")
-            cam = {k: cam[k].cpu().reshape(n_cam, -1) for k in keys}
-            lid = {k: lid[k].cpu().reshape(-1, cam[k].shape[1])[:n_lid] for k in keys}
-            cam["is_lidar"], lid["is_lidar"] = torch.zeros(n_cam, 1, dtype=torch.bool), torch.ones(n_lid, 1, dtype=torch.bool)
-            cam["sensor_idx"] = torch.zeros(n_cam, 1, dtype=torch.long)
-            lid["sensor_idx"] = torch.full((n_lid, 1), cfg.num_sensors - 1, dtype=torch.long)
-            rays = _cat(cam, lid)
+            rays, width = camera_and_lidar_rays(cfg)
         else:
             rays, width = scene.random_rays(333, cfg, seed=42), 0
         return cfg, params, _with_near_far(rays, 43), width
@@ -692,14 +698,15 @@ def level_weights64(scalings, cs64):
     return 1.0 / t.clamp_min(1.0), t
 
 
-def _level_terms(v, vabs, lw, t):
+def _level_terms(v, vabs, lw, t, k_interp=9):
     """Grid feature x = fl(trilerp fl-weights) of one level and its bound: 3 FMA-folded blends, each <= 2 U of its
-    |terms| plus U for the rounded 1 - offset (<= 9 U V_abs); the level weight by rcp.approx (<= 1 ulp = 2 U) of
-    fl(2 res std) (U) and the std's STD_REL, only where 2 res std > 1 (else exactly 1); the product U."""
+    |terms| plus U for the rounded 1 - offset (<= 9 U V_abs; `k_interp` replaces the 9 for another interpolation); the
+    level weight by rcp.approx (<= 1 ulp = 2 U) of fl(2 res std) (U) and the std's STD_REL, only where 2 res std > 1
+    (else exactly 1); the product U."""
     lw_rel = torch.where(t * (1 + STD_REL + U) > 1.0, torch.full_like(t, 3 * U + STD_REL), torch.zeros_like(t))[..., None]
     lw = lw[..., None]
     x = v * lw
-    return x, 9 * U * vabs * lw + (v * lw).abs() * (lw_rel + U)
+    return x, k_interp * U * vabs * lw + (v * lw).abs() * (lw_rel + U)
 
 
 class FieldSamples:
@@ -735,33 +742,88 @@ def _actor_tables(params, prefix, n_actors):
     return torch.stack([params[f"{prefix}.hashgrid.actor_grids.{a}.hash_table"].float() for a in range(n_actors)])
 
 
-def proposal_density_reference(params, cfg, fs, dev, drop=None):
+class TorchLayout:
+    """The reference's torch-layout field stages (hashed [L T, F] tables, one 3-D grid per actor, torch-twin SH, biased
+    nn.Linear MLPs).  The comparators take their grid, SH and parameter stages from a layout object; the walk, weights,
+    depths, appearance and actor ids do not depend on it.  tests/tcnn_trace_cases.py holds the tiny-cuda-nn layout."""
+
+    name = "torch"
+
+    def scene_rays(self, dev, name):
+        return scene_rays(dev, name)
+
+    def scene_edit(self, name):
+        return scene_edit(name)
+
+    def prop_levels(self, params, cfg, fs, dev):
+        """[(sample mask, level terms x [P_m, L], bounds)] of proposal_fields.1's static grid and actor grids."""
+        pre = "proposal_fields.1"
+        gc = cfg.proposal_grid_2
+        parts = [(fs.static, params[f"{pre}.hashgrid.static_grid.hash_table"], gc.static, fs.c32_s, fs.cs64_s, None,
+                  params[f"{pre}.hashgrid.static_grid.scalings"])]
+        if fs.R_a is not None:
+            T = gc.actor.hash_table_size
+            base = fs.aid[~fs.static] * gc.actor.num_levels * T
+            parts.append((~fs.static, _actor_tables(params, pre, cfg.n_actors), gc.actor, fs.c32_a, fs.cs64_a, base,
+                          params[f"{pre}.hashgrid.actor_grids.0.scalings"]))
+        out = []
+        for m, tab, g, c32, cs, base, sc in parts:
+            x, Ex = _level_terms(*_grid(tab, 1, g.hash_table_size, sc, c32, cs, dev, base))
+            out.append((m, x[..., 0], Ex[..., 0]))
+        return out
+
+    def main_grid(self, params, cfg, fs, dev):
+        """((static features [P_s, 32], bounds), (actor features [P_a, 16], bounds) or None)."""
+        gc = cfg.grid
+        xs, Es = _level_terms(*_grid(params["field.hashgrid.static_grid.hash_table"], 4, gc.static.hash_table_size,
+                                     params["field.hashgrid.static_grid.scalings"], fs.c32_s, fs.cs64_s, dev))
+        actor = None
+        if fs.R_a is not None:
+            T = gc.actor.hash_table_size
+            base = fs.aid[~fs.static] * gc.actor.num_levels * T
+            xa, Ea = _level_terms(*_grid(_actor_tables(params, "field", cfg.n_actors), 4, T,
+                                         params["field.hashgrid.actor_grids.0.scalings"], fs.c32_a, fs.cs64_a, dev, base))
+            actor = (xa.reshape(-1, 16), Ea.reshape(-1, 16))
+        return (xs.reshape(-1, 32), Es.reshape(-1, 32)), actor
+
+    def sh(self, dirs, E_dir, static):
+        """SH of (dir + 1) / 2 (sh4): polynomials of degree <= 3 on [0, 1]^3 whose terms are <= 3 in magnitude, <= 24 U
+        each, and Lipschitz <= 10 in the max-norm of the input."""
+        return _sh4_64((dirs + 1) / 2), 72 * U + 10 * E_dir
+
+    def linear(self, params, cfg, name, dev):
+        return params[name + ".weight"].double().to(dev), params[name + ".bias"].double().to(dev)
+
+    def lidar_layers(self, params, cfg):
+        return [(params[f"lidar_decoder.layers.{i}.weight"].double(), params[f"lidar_decoder.layers.{i}.bias"].double())
+                for i in range(3)]
+
+    def describe(self):
+        return ""
+
+
+TORCH = TorchLayout()
+
+
+def proposal_density_reference(params, cfg, fs, dev, drop=None, layout=None):
     """float64 density of proposal_fields.1 at the samples fs (static: 6 levels; actor: the actor's 4-level grid,
-    decoder inputs 0..3) and its relative bound: per level _level_terms; acc = sequential fmaf(x, dec, acc) over the L
-    levels, <= L U of sum |dec x|, plus U per term already in x; density = expf(acc): relative E_acc + 4 U.
-    `drop` = (flat sample, level): that level's term left out at that sample (a corrupted result for the self-tests)."""
+    decoder inputs 0..3) and its relative bound: per level the layout's grid terms (TorchLayout: _level_terms);
+    acc = sequential fmaf(x, dec, acc) over the L levels, <= L U of sum |dec x|, plus U per term already in x;
+    density = expf(acc): relative E_acc + 4 U.  `drop` = (flat sample, level): that level's term left out at that sample
+    (a corrupted result for the self-tests)."""
+    layout = layout or TORCH
     pre = "proposal_fields.1"
-    gc = cfg.proposal_grid_2
     dec = params[f"{pre}.density_decoder.weight"].reshape(-1).double().to(dev)
     P = fs.aid.numel()
     acc = torch.zeros(P, dtype=torch.float64, device=dev)
     E = torch.zeros_like(acc)
-    parts = [(fs.static, params[f"{pre}.hashgrid.static_grid.hash_table"], gc.static, fs.c32_s, fs.cs64_s, None,
-              params[f"{pre}.hashgrid.static_grid.scalings"])]
-    if fs.R_a is not None:
-        A, T = cfg.n_actors, gc.actor.hash_table_size
-        base = fs.aid[~fs.static] * gc.actor.num_levels * T
-        parts.append((~fs.static, _actor_tables(params, pre, A), gc.actor, fs.c32_a, fs.cs64_a, base,
-                      params[f"{pre}.hashgrid.actor_grids.0.scalings"]))
-    for m, tab, g, c32, cs, base, sc in parts:
-        v, vabs, lw, t = _grid(tab, 1, g.hash_table_size, sc, c32, cs, dev, base)
-        x, Ex = _level_terms(v, vabs, lw, t)
-        L = g.num_levels
-        terms = dec[:L] * x[..., 0]
+    for m, x, Ex in layout.prop_levels(params, cfg, fs, dev):
+        L = x.shape[-1]
+        terms = dec[:L] * x
         if drop is not None and m[drop[0]]:
             terms[int(m[:drop[0]].sum()), drop[1]] = 0.0
         acc[m.to(dev)] = terms.sum(-1)
-        E[m.to(dev)] = (dec[:L].abs() * Ex[..., 0]).sum(-1) + L * U * terms.abs().sum(-1)
+        E[m.to(dev)] = (dec[:L].abs() * Ex).sum(-1) + L * U * terms.abs().sum(-1)
     return torch.exp(acc).reshape(fs.n, fs.S).cpu(), (E + 4 * U).reshape(fs.n, fs.S).cpu()
 
 
@@ -815,7 +877,7 @@ def main_edges(cfg, bins_e_2):
     return e
 
 
-def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048, edit=None):
+def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048, edit=None, layout=None):
     """Stage 1 on every ray (actor samples through the actor's proposal grid, at the kernel's fp32 box positions, under
     the actor edit `edit`); returns (worst ratio, excl lower bounds of round 0 [n, S0])."""
     o, d, area, times = _ray_inputs(rays, idx, cfg)
@@ -828,7 +890,7 @@ def check_proposal_weights(tr, rays, idx, cfg, params, dev, chunk=2048, edit=Non
             c = slice(c0, c0 + chunk)
             fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c], edit), o[c], d[c], area[c], times[c],
                               e[c], aid[c], cfg.proposal_grid_2.actor_scale)
-            dens, rel = proposal_density_reference(params, cfg, fs, dev)
+            dens, rel = proposal_density_reference(params, cfg, fs, dev, layout=layout)
             w, tol, low = proposal_weights_reference(dens, rel, e[c])
             w_all.append(w), tol_all.append(tol), low_all.append(low)
         worst = max(worst, _ratio(tr[f"prop_weights_{rd}"], torch.cat(w_all), torch.cat(tol_all), f"prop_weights_{rd}"))
@@ -878,7 +940,7 @@ def _tf32(x):
     return (x.float().view(torch.int32) & -8192).view(torch.float32).double()
 
 
-def main_field_reference(params, cfg, fs, d, dev, gamma, corrupt=None):
+def main_field_reference(params, cfg, fs, d, dev, gamma, corrupt=None, layout=None):
     """float64 sdf [n, S] and field features [n, S, 32] at the samples fs, with per-entry bounds.
     Grid features: static 8 levels x 4, actor 4 levels x 4 padded with 16 zeros (_level_terms per entry).  Direction:
     the ray's, or for an actor sample rotated into the kernel's fp32 box frame and normalised, q / (|q| + 1e-7) (the
@@ -889,36 +951,30 @@ def main_field_reference(params, cfg, fs, d, dev, gamma, corrupt=None):
     residual geo_embedding into its accumulator (a term of its own, plus E_geo).  The sdf neuron is an fp32 FMA dot
     product over the 32 hidden units reduced over the quad, plus the bias: (32 + 3) U of sum |terms|, plus |w| E_h.
     `corrupt`: "tf32" runs the last layer as 1xTF32 (3xTF32 without its correction), "unpadded" fills an actor
-    sample's inputs 16..31 with its own features 0..15 (the self-tests)."""
+    sample's inputs 16..31 with its own features 0..15 (the self-tests).  `layout` supplies the grid features, the SH
+    basis and the MLP weights (TorchLayout by default; tests/tcnn_trace_cases.py: the tiny-cuda-nn layout)."""
+    layout = layout or TORCH
     P = fs.aid.numel()
     x = torch.zeros(P, 32, dtype=torch.float64, device=dev)
     Ex = torch.zeros_like(x)
-    gc = cfg.grid
     m = fs.static.to(dev)
-    v, vabs, lw, t = _grid(params["field.hashgrid.static_grid.hash_table"], 4, gc.static.hash_table_size,
-                           params["field.hashgrid.static_grid.scalings"], fs.c32_s, fs.cs64_s, dev)
-    xs, Es = _level_terms(v, vabs, lw, t)
-    x[m], Ex[m] = xs.reshape(-1, 32), Es.reshape(-1, 32)
+    (xs, Es), actor = layout.main_grid(params, cfg, fs, dev)
+    x[m], Ex[m] = xs, Es
     dirs = d.double()[:, None, :].expand(fs.n, fs.S, 3).reshape(-1, 3).clone().to(dev)
     E_dir = torch.full((P, 1), U, dtype=torch.float64, device=dev)
     if fs.R_a is not None:
-        T = gc.actor.hash_table_size
-        base = fs.aid[~fs.static] * gc.actor.num_levels * T
-        v, vabs, lw, t = _grid(_actor_tables(params, "field", cfg.n_actors), 4, T, params["field.hashgrid.actor_grids.0.scalings"],
-                               fs.c32_a, fs.cs64_a, dev, base)
-        xa, Ea = _level_terms(v, vabs, lw, t)
-        xa = torch.cat([xa.reshape(-1, 16), torch.zeros_like(xa.reshape(-1, 16))], 1)
+        xa, Ea = actor
+        xa = torch.cat([xa, torch.zeros_like(xa)], 1)
         if corrupt == "unpadded":
             xa[:, 16:] = xa[:, :16]
-        x[~m], Ex[~m] = xa, torch.cat([Ea.reshape(-1, 16), torch.zeros_like(Ea.reshape(-1, 16))], 1)
+        x[~m], Ex[~m] = xa, torch.cat([Ea, torch.zeros_like(Ea)], 1)
         q = (fs.R_a.double().to(dev) @ dirs[~m][..., None])[..., 0]
         dirs[~m] = q / (q.norm(dim=-1, keepdim=True) + 1e-7)
         E_dir[~m] = 16 * U
-    sh = _sh4_64((dirs + 1) / 2)
-    E_sh = 72 * U + 10 * E_dir
+    sh, E_sh = layout.sh(dirs, E_dir, m)
 
     def W(k):
-        return params[k + ".weight"].double().to(dev), params[k + ".bias"].double().to(dev)
+        return layout.linear(params, cfg, k, dev)
 
     def lin(w, b, a, Ea, extra=0.0):
         return a @ w.T + b, gamma(w.shape[1]) * (a.abs() @ w.abs().T + b.abs() + extra) + Ea @ w.abs().T
@@ -949,7 +1005,7 @@ def main_field_reference(params, cfg, fs, d, dev, gamma, corrupt=None):
     return sdf.reshape(n, S).cpu(), E_sdf.reshape(n, S).cpu(), feat.reshape(n, S, 32).cpu(), E_feat.reshape(n, S, 32).cpu()
 
 
-def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048, edit=None):
+def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048, edit=None, layout=None):
     """Stage 3: sdf and field_feature of every sample against main_field_reference at the traced bins_e_2 (the last edge
     moved to the sky), with the traced actor assignment under the actor edit `edit`.  Returns the worst ratios."""
     o, d, area, times = _ray_inputs(rays, idx, cfg)
@@ -960,7 +1016,7 @@ def check_main_field(tr, rays, idx, cfg, params, dev, gamma, chunk=2048, edit=No
         c = slice(c0, c0 + chunk)
         fs = FieldSamples(params, cfg, _frames(params, cfg, o[c], d[c], times[c], edit), o[c], d[c], area[c], times[c], e[c],
                           aid[c], cfg.grid.actor_scale)
-        sdf, Es, feat, Ef = main_field_reference(params, cfg, fs, d[c], dev, gamma)
+        sdf, Es, feat, Ef = main_field_reference(params, cfg, fs, d[c], dev, gamma, layout=layout)
         ws = max(ws, _ratio(tr["sdf"][c], sdf, Es, "sdf"))
         wf = max(wf, _ratio(tr["field_feature"][c], feat, Ef, "field_feature"))
     return {"sdf": ws, "field_feature": wf}
@@ -1023,13 +1079,12 @@ def check_actor_ids(tr, rays, idx, cfg, params, chunk=512, edit=None, corrupt=No
 
 
 # ====================================================================================== lidar head
-def check_lidar(out, cfg, params):
+def check_lidar(out, cfg, params, layout=None):
     """intensity / ray_drop_logits from the output features through the lidar decoder in float64 (lidar_decode_kernel:
     dense<> FFMA layers, gamma_ffma; intensity = 1 / (1 + expf(-o0)): relative (1 - i)(4 U) + 2 U, plus i (1 - i) E_o0)."""
     x = out["features"].double()
     E = torch.zeros_like(x)
-    for i in range(3):
-        w, b = params[f"lidar_decoder.layers.{i}.weight"].double(), params[f"lidar_decoder.layers.{i}.bias"].double()
+    for i, (w, b) in enumerate((layout or TORCH).lidar_layers(params, cfg)):
         y = x @ w.T + b
         E = gamma_ffma(w.shape[1]) * (x.abs() @ w.abs().T + b.abs()) + E @ w.abs().T
         x = y.clamp_min(0) if i < 2 else y
@@ -1061,17 +1116,19 @@ def select(out, idx):
     return {k: v[idx.to(v.device)].cpu() for k, v in out.items()}
 
 
-def check_scene(dev, name, mode="split", n_random=127, report=print, gamma=None):
+def check_scene(dev, name, mode="split", n_random=127, report=print, gamma=None, layout=None):
     """Full trace of one scene: every stage on whole 128-ray warp groups (every ray on the CPU); then a render with a
     partial trace (no actor ids: the early exit on) and an untraced render must match the full trace bit for bit.
     `gamma`: the MLP's per-term constant of the main-field bounds; by default the one of the MLP that ran, gamma_ffma
-    in the emulation and gamma_f16 for the lane kernels' fp16 split on the GPU.
+    in the emulation and gamma_f16 for the lane kernels' fp16 split on the GPU.  `layout`: the parameter layout whose
+    scenes, grids, SH and MLPs the field stages use (TorchLayout by default).
     Returns (worst ratio per stage, inferred early-exit warps, actor-id face exceptions, full render, referenced rays)."""
     t0 = time.perf_counter()
+    layout = layout or TORCH
     if gamma is None:
         gamma = gamma_ffma if dev == "cpu" else gamma_f16
-    cfg, params, rays, width = scene_rays(dev, name)
-    edit = scene_edit(name)
+    cfg, params, rays, width = layout.scene_rays(dev, name)
+    edit = layout.scene_edit(name)
     r = renderer(dev, cfg, params, edit)
     rd = {k: (v.to(dev) if dev != "cpu" else v) for k, v in rays.items()}
     full = r.render(rd, want_trace=True, image_width=width, mode=mode, want_intensity=True)
@@ -1086,17 +1143,17 @@ def check_scene(dev, name, mode="split", n_random=127, report=print, gamma=None)
     check_walk(out, rays, idx, cfg)
     worst.update(check_shading(out, out, rays, idx, cfg, params))
     fdev = "cpu" if dev == "cpu" else dev
-    worst["prop_weights"], low = check_proposal_weights(out, rays, idx, cfg, params, fdev, edit=edit)
-    worst.update(check_main_field(out, rays, idx, cfg, params, fdev, gamma, edit=edit))
+    worst["prop_weights"], low = check_proposal_weights(out, rays, idx, cfg, params, fdev, edit=edit, layout=layout)
+    worst.update(check_main_field(out, rays, idx, cfg, params, fdev, gamma, edit=edit, layout=layout))
     if "intensity" in out:
-        worst.update(check_lidar(out, cfg, params))
+        worst.update(check_lidar(out, cfg, params, layout))
     exits = early_exit_warps(low, idx) if width == 0 else 0
     faces = 0
     if cfg.n_actors:
         hits = int((out["actor_id_main"] >= 0).sum())
         # sweeps are not aimed at the boxes: the GPU's three 32-beam sweeps put ~600 samples in them, the golden's viewer
-        # sweep (8 beams, 7.5 degree columns) a handful
-        need = max(10, n // 40) if not name.startswith("sweep") else 0 if dev == "cpu" else 300
+        # sweep (8 beams, 7.5 degree columns) a handful; a camera image (width > 0) holds its aimed rays after the image
+        need = max(10, n // 40) if "sweep" not in name and not width else 0 if dev == "cpu" else 300
         assert hits >= need, f"{name}: only {hits} actor samples: the actor branch is not exercised"
         faces, _ = check_actor_ids(out, rays, idx, cfg, params, edit=edit)
         for a in edit_selection(cfg.n_actors, edit):
@@ -1112,5 +1169,6 @@ def check_scene(dev, name, mode="split", n_random=127, report=print, gamma=None)
         _bits_equal(none[k], full[k].cpu(), f"{name} {mode}: untraced output {k}")
     report(f"\n[render trace] {name} {mode}: {idx.numel()} of {n} rays referenced; worst |got - ref| / bound: "
            + ", ".join(f"{k} {v:.3g}" for k, v in worst.items())
-           + f"; early-exit warps (inferred) {exits}; actor-id face exceptions {faces}; {time.perf_counter() - t0:.1f} s")
+           + f"; early-exit warps (inferred) {exits}; actor-id face exceptions {faces}{layout.describe()}; "
+           + f"{time.perf_counter() - t0:.1f} s")
     return worst, exits, faces, full, idx
