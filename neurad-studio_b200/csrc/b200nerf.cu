@@ -282,7 +282,9 @@ static auto sample_lane_kernel(bool actors, bool traced, bool edit) {
                   : nff_sample_lane_kernel<LAYOUT, false, false, false>;
 }
 
-template <int LAYOUT, bool EDIT>
+// ACTORS = false: the scene has no actors; the actor path is left out and the SH encoding is set once per ray
+// (shade_ray_lane).  Trace stores stay runtime-tested in every instance.
+template <int LAYOUT, bool ACTORS, bool EDIT>
 __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_kernel(const __grid_constant__ RenderParams P,
                                                                                       float* __restrict__ scratch,
                                                                                       const float* __restrict__ handoff) {
@@ -319,9 +321,17 @@ __global__ void __launch_bounds__(kLaneThreads, kLaneCtasPerSm) nff_shade_lane_k
     }
     int64_t ray;
     const bool active = lane_patch_ray(P, patch, tid & 31, &ray);
-    const LaneRay R = lane_ray_setup<true, EDIT>(P, sc, tid, ray);
-    shade_ray_lane<MlpLaneTc, LAYOUT>(P, sc, R, mlp, tid, ray, active, handoff + ray, P.n_rays);
+    const LaneRay R = lane_ray_setup<ACTORS, EDIT>(P, sc, tid, ray);
+    shade_ray_lane<MlpLaneTc, LAYOUT, ACTORS>(P, sc, R, mlp, tid, ray, active, handoff + ray, P.n_rays);
   }
+}
+// the instance of a launch, by sample_lane_kernel's rule: `actors` = the scene has actors, `edit` = an actor edit is
+// active (the scene has actors)
+template <int LAYOUT>
+static auto shade_lane_kernel(bool actors, bool edit) {
+  return edit ? nff_shade_lane_kernel<LAYOUT, true, true>
+         : actors ? nff_shade_lane_kernel<LAYOUT, true, false>
+                  : nff_shade_lane_kernel<LAYOUT, false, false>;
 }
 
 // Ray-per-lane variant (nff_lane.h), single fused kernel: a warp = 32 adjacent rays at the same sample index.
@@ -1076,9 +1086,9 @@ int b200nerf_create(int device_ordinal, b200nerf_ctx** out) {
     CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lane_tc_smem_bytes()));
   c->lane_ctas = c->sm_count * (kLaneCtasPerSm > NFF_SAMPLE_CTAS ? kLaneCtasPerSm : NFF_SAMPLE_CTAS);
   CUDA_TRY(cudaMalloc((void**)&c->d_lane_scratch, sizeof(float) * lane_scratch_floats_per_cta() * c->lane_ctas));
-  for (auto k : {nff_shade_lane_kernel<0, false>, nff_shade_lane_kernel<1, false>, nff_shade_lane_kernel<0, true>,
-                 nff_shade_lane_kernel<1, true>})
-    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lane_tc_smem_bytes()));
+  for (int i = 0; i < 4; ++i)
+    for (auto k : {shade_lane_kernel<0>(i & 1, i & 2), shade_lane_kernel<1>(i & 1, i & 2)})
+      CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lane_tc_smem_bytes()));
   // (almost) all L1: the smallest carve-out that holds the 516 B edge table of each resident CTA
   for (int i = 0; i < 8; ++i) {
     CUDA_TRY(cudaFuncSetAttribute(sample_lane_kernel<0>(i & 1, i & 2, i & 4), cudaFuncAttributePreferredSharedMemoryCarveout, 0));
@@ -1487,12 +1497,10 @@ int b200nerf_nff_render_fwd(b200nerf_ctx* c, const b200nerf_rays* rays, int64_t 
       const bool actors = c->actors.n_actors > 0;
       if (c->layout == 1) {
         sample_lane_kernel<1>(actors, traced, edit)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
-        (edit ? nff_shade_lane_kernel<1, true> : nff_shade_lane_kernel<1, false>)<<<(int)grid_b, kLaneThreads, smem, st>>>(
-            Q, c->d_lane_scratch, c->d_handoff);
+        shade_lane_kernel<1>(actors, edit)<<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
       } else {
         sample_lane_kernel<0>(actors, traced, edit)<<<(int)grid_a, kLaneThreads, 0, st>>>(Q, c->d_lane_scratch, c->d_handoff);
-        (edit ? nff_shade_lane_kernel<0, true> : nff_shade_lane_kernel<0, false>)<<<(int)grid_b, kLaneThreads, smem, st>>>(
-            Q, c->d_lane_scratch, c->d_handoff);
+        shade_lane_kernel<0>(actors, edit)<<<(int)grid_b, kLaneThreads, smem, st>>>(Q, c->d_lane_scratch, c->d_handoff);
       }
     }
   } else if (c->mlp_mode == 2) {

@@ -428,9 +428,10 @@ NFF_D float tcnn_encode_f1_dot(const Grid& gr, int L, const float* x, float std,
   }
   return acc;
 }
-// F = 4 grid into a strided column (the tcnn twin of encode_f4_col / encode_f4_panel): out[(4l+f) * stride]
+// F = 4 grid into a strided column (the tcnn twin of encode_f4_col / encode_f4_panel): out[(4l+f) * stride], times
+// `scale` (a power of two: the stored values are exactly `scale` times the features)
 template <int D>
-NFF_D void tcnn_encode_f4(const Grid& gr, int L, const float* x, float std, float* out, int stride) {
+NFF_D void tcnn_encode_f4(const Grid& gr, int L, const float* x, float std, float* out, int stride, float scale) {
 #pragma unroll 1
   for (int l = 0; l < L; ++l) {
     uint32_t idx[1 << D];
@@ -449,7 +450,7 @@ NFF_D void tcnn_encode_f4(const Grid& gr, int L, const float* x, float std, floa
       a2 = fmaf(w, v[c].z, a2);
       a3 = fmaf(w, v[c].w, a3);
     }
-    const float lw = level_weight(gr.res[l], std);
+    const float lw = fmul(level_weight(gr.res[l], std), scale);
     out[(4 * l + 0) * stride] = fmul(a0, lw);
     out[(4 * l + 1) * stride] = fmul(a1, lw);
     out[(4 * l + 2) * stride] = fmul(a2, lw);

@@ -179,8 +179,10 @@ NFF_D float lane_proposal_density(const FieldGrids& fg, const LaneScratch& sc, i
   return expf(acc);
 }
 
-// F = 4 grid into the CTA's shared panel column [4l+f][tid] (rolled level loop: small code); `pitch` = panel row pitch
-NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L, Gauss g, float* x /* = panel + tid */, int pitch) {
+// F = 4 grid into the CTA's shared panel column [4l+f][tid] (rolled level loop: small code); `pitch` = panel row pitch.
+// The stored values are `scale` (a power of two, folded into the level weight) times the features, exactly.
+NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L, Gauss g, float* x /* = panel + tid */, int pitch,
+                         float scale) {
   const uint32_t maskb = gr.mask << 4;
 #pragma unroll 2
   for (int l = 0; l < L; ++l) {
@@ -192,7 +194,7 @@ NFF_D void encode_f4_col(const float* NFF_RESTRICT table, const Grid& gr, int L,
     float4 v[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) v[k] = ldg_at<float4>(base, r[k]);
-    float w = level_weight(res, g.std);
+    const float w = fmul(level_weight(res, g.std), scale);
     const float ix = 1.0f - c.ox, iy = 1.0f - c.oy, iz = 1.0f - c.oz;
 #if NFF_F4_WEIGHTS
     // the 8 corner weights are shared by the row's 4 features: 14 multiplies for the weights (level weight folded in) and
@@ -323,21 +325,29 @@ NFF_D float lane_proposal_round(const RenderParams& P, const FieldGrids& fg, con
 }
 
 // ------------------------------------------------------------------------------------------- MLP policies, per lane
-// Input: the 32 grid features of this lane's sample in registers.  CUDA-core version (host emulation / fp32 mode):
+// Input: the 32 grid features of this lane's sample in registers, kAScale times the features (the grid encoders write
+// the panel at that scale); the direction's SH encoding from the last set_dir.  CUDA-core version (host emulation / fp32
+// mode):
 struct MlpLaneFfma {
   static constexpr int kPitch = kLaneThreads;  // panel row pitch (floats)
+  static constexpr float kAScale = 1.0f;
   const float* w;  // packed transposed weights (nff_params.h)
   float* panel_;   // [kNff][kLaneThreads]
   int sh_tcnn = 0;  // 1: tiny-cuda-nn's SphericalHarmonics convention (nff_device.h: sh4_tcnn)
+  float sh_[kSh] = {};
   NFF_D float* panel() const { return panel_; }
-  NFF_D void run(const float* x, const float dir[3], float& sdf, float* feat, int /*tid*/) const {
+  NFF_D void set_dir(const float dir[3], int /*tid*/) {
+    if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], sh_); else sh4(dir[0], dir[1], dir[2], sh_);
+  }
+  NFF_D void run(const float* x, float& sdf, float* feat, int /*tid*/) const {
     float h[kHidden], go[kNff + 1], in2[kNff + kSh], h2[kHidden];
     dense<kGeoIn, kHidden, kHidden, true>(w + kOffGeoW0, w + kOffGeoB0, x, h);
     dense<kHidden, kNff + 1, kGeoOutP, false>(w + kOffGeoW1, w + kOffGeoB1, h, go);
     sdf = go[0];
 #pragma unroll
     for (int i = 0; i < kNff; ++i) in2[i] = go[i + 1];
-    if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], in2 + kNff); else sh4(dir[0], dir[1], dir[2], in2 + kNff);
+#pragma unroll
+    for (int i = 0; i < kSh; ++i) in2[kNff + i] = sh_[i];
     dense<kNff + kSh, kHidden, kHidden, true>(w + kOffFeatW0, w + kOffFeatB0, in2, h);
     dense<kHidden, kHidden, kHidden, true>(w + kOffFeatW1, w + kOffFeatB1, h, h2);
     dense<kHidden, kNff, kNff, false>(w + kOffFeatW2, w + kOffFeatB2, h2, h);
@@ -353,19 +363,22 @@ struct MlpLaneFfma {
 //         a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo        (hi = x rounded to fp16, lo = x - hi rounded to fp16)
 //     three wgmma per k16 step (DESIGN section 4 bounds it);
 //   * the operands are scaled by powers of two to sit inside fp16's range: A by 2^kLaneTcA, layer l's B by 2^e_l, chosen
-//     from the layer's largest weight when the tiles are staged.  Accumulators start at the bias times 2^(kLaneTcA + e_l)
-//     and are scaled back exactly (by 2^-e_l) before ReLU, so the next layer's A is 2^kLaneTcA times the activation;
+//     from the layer's largest weight when the tiles are staged.  Each layer's first wgmma starts its accumulators at zero
+//     (scale-d = 0); after the wait one FMA per accumulator scales the products back exactly (by 2^-e_l) and adds the bias
+//     times 2^kLaneTcA, so the next layer's A is 2^kLaneTcA times the activation;
 //   * layer 0 loads its A fragments straight from the grid-feature panel (rows 0..31; a row pitch of 4 mod 32 banks keeps
 //     those loads free of bank conflicts).  Layer 2's K columns 32..47, the SH encoding of the direction, come from panel
-//     rows 32..47, which the row owner writes next to its features before the group barrier;
+//     rows 32..47, which the row owner writes (set_dir) before the group barrier.  The writers store both already times
+//     2^kLaneTcA (kAScale), so the fragments are the A operands as loaded;
 //   * layers 1-4 take the previous layer's accumulator registers as their A operand: the fp32 accumulator fragment of an
 //     m64nN wgmma (rows g / g+8, columns 8j+2t, +1) is the register A fragment of an f16 k16 step, pair by pair;
-//   * accumulators start at the bias, layer 4's at bias + geo_embedding (the residual).  geo_embedding waits in the panel
-//     at the thread's own fragment positions (rows 0..31, consumed by layer 0) while layers 2-3 run;
+//   * layer 4's products are scaled by 2^-(kLaneTcA + e_4) in the same FMA that adds bias + geo_embedding (the
+//     residual).  geo_embedding waits in the panel at the thread's own fragment positions (rows 0..31, consumed by layer 0)
+//     while layers 2-3 run;
 //   * the sdf neuron is a dot product of layer 0's fragments: 8 terms per thread, then a reduction over the quad;
 //   * one commit and one wait per layer and half: 10 waits per sample;
-//   * an A operand at or beyond fp16's overflow threshold would turn into inf inside the product: each layer checks its
-//     largest scaled operand and raises P.status (kLaneTcRangeStatus) instead.
+//   * an A operand at or beyond fp16's overflow threshold would turn into inf inside the product: each layer checks the
+//     largest of its packed fp16 hi words and raises P.status (kLaneTcRangeStatus) instead.
 // The outputs (feature c of tile row R at panel[c][R], sdf at panel[48][R]) reach the row owner behind the second and
 // last group barrier of the sample.  Panel positions of a tile row are only ever read and written as fragments by the
 // warp whose fragments hold that row, and by the row owner on the far side of a barrier.
@@ -377,9 +390,10 @@ constexpr float kLaneTcOverflow = 65520.0f;       // the smallest fp32 value tha
 constexpr int kLaneTcRangeStatus = 4;             // P.status code: an MLP activation beyond the fp16 operand range
 struct LaneTcShared {
   __half b[2 * 32 * (32 + 32 + 48 + 32 + 32)];  // hi|lo fp16 B tiles of the 5 layers, layer l times 2^e_l (22 KiB)
-  float bias[kTcLayers][32];                     // times 2^(kLaneTcA + e_l)
-  float up[kTcLayers], down[kTcLayers];          // 2^e_l, 2^-e_l
-  float w_sdf[32];
+  // bias and w_sdf are read as float2 fragments (8-byte aligned)
+  alignas(8) float bias[kTcLayers][32];          // layers 0-3 times 2^kLaneTcA; layer 4 as it is (added to its output)
+  float down[kTcLayers];                         // 2^-e_l
+  alignas(8) float w_sdf[32];
   float b_sdf;
   unsigned wmax[kTcLayers];                      // staging: the bits of the largest |weight| of each layer
 };
@@ -408,8 +422,8 @@ NFF_D void lane_tc_stage_weights(LaneTcShared& t, const float* NFF_RESTRICT nn, 
     const int K = tc_layer_k(l);
     __half* hi = t.b + tc_layer_off(l);
     tc::stage_b_tile_f16(hi, hi + 32 * K, nn + tc_layer_w(l), K, up, tid, nthreads);
-    for (int i = tid; i < 32; i += nthreads) t.bias[l][i] = nn[tc_layer_b(l) + i] * up * kLaneTcAScale;
-    if (tid == 0) t.up[l] = up, t.down[l] = down;
+    for (int i = tid; i < 32; i += nthreads) t.bias[l][i] = nn[tc_layer_b(l) + i] * (l < kTcLayers - 1 ? kLaneTcAScale : 1.0f);
+    if (tid == 0) t.down[l] = down;
   }
   for (int i = tid; i < 32; i += nthreads) t.w_sdf[i] = nn[kNnGeoW1 + i];
   if (tid == 0) t.b_sdf = nn[kNnGeoB1];
@@ -417,6 +431,7 @@ NFF_D void lane_tc_stage_weights(LaneTcShared& t, const float* NFF_RESTRICT nn, 
 
 struct MlpLaneTc {
   static constexpr int kPitch = kLanePanelPitch;
+  static constexpr float kAScale = kLaneTcAScale;  // the panel's grid features and SH are the scaled A operands
   const LaneTcShared* t;  // staged by lane_tc_stage_weights; at the start of dynamic shared memory
   float* panel_;          // [kLanePanelRows][kPitch] shared memory
   int* status;            // RenderParams::status
@@ -434,19 +449,22 @@ struct MlpLaneTc {
     return tc::smem_desc_lo(tc::smem_u32(nff_lane_smem + offsetof(LaneTcShared, b)), 128u);
   }
 
-  // acc (this thread's 16 fragment registers of one m64n32 half, preset by the caller) += A * W^T over the KS k16 steps
-  // of a layer with K inputs; a = the scaled A operands, 8 per k-step in fragment order; OFF = the half offset in t->b of
-  // the layer's hi B tile (lo follows it).  Every descriptor is b_desc_lo() plus a compile-time constant.
+  // acc (this thread's 16 fragment registers of one m64n32 half) = A * W^T over the KS k16 steps of a layer with K inputs
+  // (the first wgmma starts from zero); a = the scaled A operands, 8 per k-step in fragment order; OFF = the half offset in
+  // t->b of the layer's hi B tile (lo follows it).  Every descriptor is b_desc_lo() plus a compile-time constant.
   template <int KS, int K, int OFF>
   NFF_D void half_mma(float* acc, const float* a) const {
     uint32_t ah[4 * KS], al[4 * KS];
-    float amax = 0.0f;
+    // Range check on the packed hi words: with round-to-nearest-even rn16(x) is inf exactly when |x| >= kLaneTcOverflow.
+    // __hmax2 returns the other operand where one is NaN, so a NaN operand does not raise the status (as fmaxf did not).
+    __half2 amax = __float2half2_rn(0.0f);
 #pragma unroll
     for (int i = 0; i < 4 * KS; ++i) {
-      amax = fmaxf(amax, fmaxf(fabsf(a[2 * i]), fabsf(a[2 * i + 1])));
       tc::f16x2_split(a[2 * i], a[2 * i + 1], ah[i], al[i]);
+      amax = __hmax2(amax, __habs2(*reinterpret_cast<const __half2*>(&ah[i])));
     }
-    if (amax >= kLaneTcOverflow && status) atomicExch(status, kLaneTcRangeStatus);
+    if (__hge2_mask(amax, __half2half2(__ushort_as_half((unsigned short)0x7c00u))) != 0u && status)  // either half is inf
+      atomicExch(status, kLaneTcRangeStatus);
     constexpr uint32_t sbo = (uint32_t)(K / 8) * 128u;  // (K / 8) core matrices of 128 B per 8-row n block
     constexpr uint32_t hi_off = (uint32_t)OFF * 2u / 16u, lo_off = (uint32_t)(OFF + 32 * K) * 2u / 16u;
     const uint32_t b_desc = b_desc_lo();
@@ -455,7 +473,8 @@ struct MlpLaneTc {
     for (int ks = 0; ks < KS; ++ks) {
       const uint32_t adv = (uint32_t)(ks * 2 * 128) / 16u;  // two 16-byte K-chunks per k-step
       const uint64_t dh = tc::smem_desc_of(b_desc + hi_off + adv, sbo), dl = tc::smem_desc_of(b_desc + lo_off + adv, sbo);
-      tc::wgmma_f16_m64n32(acc, ah + 4 * ks, dh);
+      if (ks == 0) tc::wgmma_f16_m64n32_zero(acc, ah, dh);
+      else tc::wgmma_f16_m64n32(acc, ah + 4 * ks, dh);
       tc::wgmma_f16_m64n32(acc, al + 4 * ks, dh);
       tc::wgmma_f16_m64n32(acc, ah + 4 * ks, dl);
     }
@@ -471,42 +490,44 @@ struct MlpLaneTc {
 #pragma unroll
     for (int i = 0; i < n; ++i) {
       const float* r = p + (16 * (ks0 + i) + 2 * q) * kPitch;
-      a[8 * i + 0] = r[0] * kLaneTcAScale;
-      a[8 * i + 1] = r[kPitch] * kLaneTcAScale;
-      a[8 * i + 2] = r[8] * kLaneTcAScale;
-      a[8 * i + 3] = r[kPitch + 8] * kLaneTcAScale;
-      a[8 * i + 4] = r[8 * kPitch] * kLaneTcAScale;
-      a[8 * i + 5] = r[9 * kPitch] * kLaneTcAScale;
-      a[8 * i + 6] = r[8 * kPitch + 8] * kLaneTcAScale;
-      a[8 * i + 7] = r[9 * kPitch + 8] * kLaneTcAScale;
+      a[8 * i + 0] = r[0];
+      a[8 * i + 1] = r[kPitch];
+      a[8 * i + 2] = r[8];
+      a[8 * i + 3] = r[kPitch + 8];
+      a[8 * i + 4] = r[8 * kPitch];
+      a[8 * i + 5] = r[9 * kPitch];
+      a[8 * i + 6] = r[8 * kPitch + 8];
+      a[8 * i + 7] = r[9 * kPitch + 8];
     }
   }
-  NFF_D static void bias_init(float* acc, const float* bias, int q) {
+  // accumulators times 2^-e_l (exact) plus 2^kLaneTcA times the bias: 2^kLaneTcA times the layer's output
+  NFF_D static void rescale_bias(float* acc, float down, const float* bias, int q) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q);
-      acc[4 * j + 0] = acc[4 * j + 2] = b.x;
-      acc[4 * j + 1] = acc[4 * j + 3] = b.y;
+      acc[4 * j + 0] = fmaf(acc[4 * j + 0], down, b.x);
+      acc[4 * j + 1] = fmaf(acc[4 * j + 1], down, b.y);
+      acc[4 * j + 2] = fmaf(acc[4 * j + 2], down, b.x);
+      acc[4 * j + 3] = fmaf(acc[4 * j + 3], down, b.y);
     }
-  }
-  // accumulators times 2^-e_l: 2^kLaneTcA times the layer's output (exact)
-  NFF_D static void unscale(float* acc, float down) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) acc[i] *= down;
   }
   NFF_D static void relu(float* acc) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) acc[i] = fmaxf(acc[i], 0.0f);
   }
 
-  NFF_D void run(const float* /* x: read as fragments from the panel */, const float dir[3], float& sdf, float* feat, int tid) {
+  // SH encoding of the shading direction, times 2^kLaneTcA, into panel rows 32..47 of this thread's column.  Only layer 2's
+  // fragment loads read those rows, and nothing else writes them: the next run's first group barrier orders the writes.
+  NFF_D void set_dir(const float dir[3], int tid) const {
+    float shv[kSh];
+    if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], shv); else sh4(dir[0], dir[1], dir[2], shv);
     float* col = panel_ + tid;
-    {
-      float shv[kSh];
-      if (sh_tcnn) sh4_tcnn(dir[0], dir[1], dir[2], shv); else sh4(dir[0], dir[1], dir[2], shv);
 #pragma unroll
-      for (int i = 0; i < kSh; ++i) col[(kGeoIn + i) * kPitch] = shv[i];
-    }
+    for (int i = 0; i < kSh; ++i) col[(kGeoIn + i) * kPitch] = shv[i] * kLaneTcAScale;
+  }
+
+  NFF_D void run(const float* /* x: read as fragments from the panel */, float& sdf, float* feat, int tid) {
+    float* col = panel_ + tid;
     group_sync();  // all 128 panel columns of the group are in
     const int ln = tid & 31, q = ln & 3;
     // accumulator fragment (row g (+8), columns 8j + 2q (+1)) of tile row 64h + 16 warp + g: panel column fr + 64 h
@@ -517,9 +538,8 @@ struct MlpLaneTc {
       float a[24], acc[16];
       // layer 0: grid features -> hidden, ReLU, sdf
       load_a(a, p, q, 0, 2);
-      bias_init(acc, t->bias[0], q);
       half_mma<2, 32, tc_layer_off(0)>(acc, a);
-      unscale(acc, t->down[0]);
+      rescale_bias(acc, t->down[0], t->bias[0], q);
       relu(acc);
       float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
@@ -539,9 +559,8 @@ struct MlpLaneTc {
       // layer 1: -> geo_embedding (scaled), parked at this thread's fragment positions of panel rows 0..31
 #pragma unroll
       for (int i = 0; i < 16; ++i) a[i] = acc[i];
-      bias_init(acc, t->bias[1], q);
       half_mma<2, 32, tc_layer_off(1)>(acc, a);
-      unscale(acc, t->down[1]);
+      rescale_bias(acc, t->down[1], t->bias[1], q);
       __syncwarp();  // the warp's layer-0 fragment loads of these rows are done
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -552,34 +571,28 @@ struct MlpLaneTc {
 #pragma unroll
       for (int i = 0; i < 16; ++i) a[i] = acc[i];
       load_a(a + 16, p, q, 2, 1);
-      bias_init(acc, t->bias[2], q);
       half_mma<3, 48, tc_layer_off(2)>(acc, a);
-      unscale(acc, t->down[2]);
+      rescale_bias(acc, t->down[2], t->bias[2], q);
       relu(acc);
       // layer 3: hidden -> hidden, ReLU
 #pragma unroll
       for (int i = 0; i < 16; ++i) a[i] = acc[i];
-      bias_init(acc, t->bias[3], q);
       half_mma<2, 32, tc_layer_off(3)>(acc, a);
-      unscale(acc, t->down[3]);
+      rescale_bias(acc, t->down[3], t->bias[3], q);
       relu(acc);
-      // layer 4: hidden -> features, accumulated onto bias + geo_embedding; out to the same positions
+      // layer 4: hidden -> features, products times 2^-(kLaneTcA + e_4) plus bias + geo_embedding; out to the same positions
 #pragma unroll
       for (int i = 0; i < 16; ++i) a[i] = acc[i];
-      bias_init(acc, t->bias[4], q);
-      const float up4 = t->up[4], out4 = t->down[4] * kLaneTcAUnscale;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float* r = p + (8 * j + 2 * q) * kPitch;
-        acc[4 * j + 0] += r[0] * up4, acc[4 * j + 1] += r[kPitch] * up4;
-        acc[4 * j + 2] += r[8] * up4, acc[4 * j + 3] += r[kPitch + 8] * up4;
-      }
       half_mma<2, 32, tc_layer_off(4)>(acc, a);
+      const float out4 = t->down[4] * kLaneTcAUnscale;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         float* r = p + (8 * j + 2 * q) * kPitch;
-        r[0] = acc[4 * j + 0] * out4, r[kPitch] = acc[4 * j + 1] * out4;
-        r[8] = acc[4 * j + 2] * out4, r[kPitch + 8] = acc[4 * j + 3] * out4;
+        const float2 b = *reinterpret_cast<const float2*>(t->bias[4] + 8 * j + 2 * q);
+        r[0] = fmaf(acc[4 * j + 0], out4, fmaf(r[0], kLaneTcAUnscale, b.x));
+        r[kPitch] = fmaf(acc[4 * j + 1], out4, fmaf(r[kPitch], kLaneTcAUnscale, b.y));
+        r[8] = fmaf(acc[4 * j + 2], out4, fmaf(r[8], kLaneTcAUnscale, b.x));
+        r[kPitch + 8] = fmaf(acc[4 * j + 3], out4, fmaf(r[kPitch + 8], kLaneTcAUnscale, b.y));
       }
     }
     group_sync();  // every tile row's outputs are in
@@ -665,7 +678,9 @@ NFF_D void sample_ray_lane(const RenderParams& P, const LaneScratch& sc, const L
 }
 
 // Shading stage: main field on the 32 resampled intervals + compositing + outputs (neurad.py:368-401).
-template <class Mlp, int LAYOUT = 0>
+// ACTORS = false: the scene has no actors (n_cand == 0).  The actor path is not compiled in, and the shading direction is
+// the ray's own for every sample, so its SH encoding is set once per ray.
+template <class Mlp, int LAYOUT = 0, bool ACTORS = true>
 NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const LaneRay& R, Mlp& mlp, int tid, int64_t ray,
                           bool active, const float* bins2, int64_t bins2_stride) {
   const Sampling& sp = P.samp;
@@ -682,6 +697,7 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
   double T_d = 1.0;
   float acc = 0.0f, depth = 0.0f;
   float e_prev = to_euclid(bins2[0], s_near, s_far, sp);
+  if (!ACTORS) mlp.set_dir(d, tid);
 #pragma unroll 1
   for (int s = 0; s < kS2; ++s) {
     const float e0 = e_prev;
@@ -690,11 +706,11 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
     if (s == kS2 - 1) e1 = fadd(e1, fsub(sp.sky_distance, e1));  // sky sample (neurad.py:451-455)
     Gauss g = sample_gaussian(o, d, area, e0, e1);
     float* col = mlp.panel() + tid;  // this thread's column of the [32][Mlp::kPitch] shared panel
-    float dir[3] = {d[0], d[1], d[2]};
     int aid = -1;
     {
+      float dir[3] = {d[0], d[1], d[2]};
       float pb[3], M[12];
-      aid = n_cand > 0 ? lane_actor_of_sample(sc, tid, n_cand, g, pb, M) : -1;
+      if (ACTORS && n_cand > 0) aid = lane_actor_of_sample(sc, tid, n_cand, g, pb, M);
       if (aid >= 0) {
         Gauss ga = {pb[0], pb[1], pb[2], g.std};
         ga = contract(ga, fm.actor_scale);
@@ -702,9 +718,9 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
         for (int i = 16; i < 32; ++i) col[i * Mlp::kPitch] = 0.0f;  // F.pad(actor_features, (0, 32-16))
         if (LAYOUT == 1) {
           const float x4[4] = {ga.x, ga.y, ga.z, fdiv((float)aid, fm.n_actors_f)};
-          tcnn_encode_f4<4>(fm.act, 4, x4, ga.std, col, Mlp::kPitch);
+          tcnn_encode_f4<4>(fm.act, 4, x4, ga.std, col, Mlp::kPitch, Mlp::kAScale);
         } else {
-          encode_f4_col(fm.actor_tables[aid], fm.act, 4, ga, col, Mlp::kPitch);
+          encode_f4_col(fm.actor_tables[aid], fm.act, 4, ga, col, Mlp::kPitch, Mlp::kAScale);
         }
         float q0 = fadd(fadd(fmul(M[0], d[0]), fmul(M[1], d[1])), fmul(M[2], d[2]));
         float q1 = fadd(fadd(fmul(M[4], d[0]), fmul(M[5], d[1])), fmul(M[6], d[2]));
@@ -715,17 +731,18 @@ NFF_D void shade_ray_lane(const RenderParams& P, const LaneScratch& sc, const La
         Gauss gs = contract(g, fm.static_scale);
         if (LAYOUT == 1) {
           const float x3[3] = {gs.x, gs.y, gs.z};
-          tcnn_encode_f4<3>(fm.stat, 8, x3, gs.std, col, Mlp::kPitch);
+          tcnn_encode_f4<3>(fm.stat, 8, x3, gs.std, col, Mlp::kPitch, Mlp::kAScale);
         } else {
-          encode_f4_col(fm.stat.table, fm.stat, 8, gs, col, Mlp::kPitch);
+          encode_f4_col(fm.stat.table, fm.stat, 8, gs, col, Mlp::kPitch, Mlp::kAScale);
         }
       }
+      if (ACTORS) mlp.set_dir(dir, tid);
     }
     float x[kGeoIn];
 #pragma unroll
     for (int i = 0; i < kGeoIn; ++i) x[i] = col[i * Mlp::kPitch];
     float sdf, feat[kNff];
-    mlp.run(x, dir, sdf, feat, tid);
+    mlp.run(x, sdf, feat, tid);
     const float alpha = frcp(fadd(1.0f, expf(fmul(sdf, P.beta))));
     float w = fmul(alpha, (float)T_d);  // nerfacc.render_weight_from_alpha, torch.cumprod order
     T_d *= (double)fsub(1.0f, alpha);

@@ -120,6 +120,14 @@ __device__ __forceinline__ void wgmma_f16_m64n32(float* d, const uint32_t* a, ui
                : TC_D16(0)
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
 }
+// the same with scale-d = 0: D = A * B, the accumulators' previous values are not read
+__device__ __forceinline__ void wgmma_f16_m64n32_zero(float* d, const uint32_t* a, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+               : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]),
+                 "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(0));
+}
 template <int N>
 __device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t b_desc) {
   static_assert(N == 16 || N == 32 || N == 48 || N == 64, "tf32 tile widths");
