@@ -545,8 +545,9 @@ class FeatureRenderer(nn.Module):
 
 
 class RGBRenderer(nn.Module):
-    """model_components/renderers.py:93-268 in eval mode: nan_to_num(rgb), composite, blend a constant background
-    ("random" / None = no blending, like black; "last_sample" is not provided)."""
+    """model_components/renderers.py:93-268: composite and blend a constant background ("random" / None = no blending,
+    like black; "last_sample" is not provided).  In eval mode the samples' rgb go through nan_to_num first and the
+    result is clamped to [0, 1]; in training mode neither (renderers.py:258-265)."""
 
     COLORS = {"white": (1.0, 1.0, 1.0), "black": (0.0, 0.0, 0.0), "red": (1.0, 0.0, 0.0), "green": (0.0, 1.0, 0.0),
               "blue": (0.0, 0.0, 1.0)}  # utils/colors.py:21-31
@@ -565,7 +566,8 @@ class RGBRenderer(nn.Module):
         elif isinstance(bg, Tensor):
             bg = [float(v) for v in bg.reshape(-1)]
         be = get_backend(weights.device)
-        return be.composite(weights, rgb, background=bg, value_nan_to_num=True, want_accumulation=False)["values"]
+        out = be.composite(weights, rgb, background=bg, value_nan_to_num=not self.training, want_accumulation=False)["values"]
+        return out if self.training else out.clamp_(0.0, 1.0)
 
     def forward(self, rgb: Tensor, weights: Tensor) -> Tensor:
         _no_backward("RGBRenderer", rgb, weights)

@@ -86,14 +86,15 @@ def mlp_forward(weights, biases, x: Tensor) -> Tensor:
     return x
 
 
-def rgb_render(rgb: Tensor, weights: Tensor, background: Optional[Tensor]) -> Tensor:
-    """RGBRenderer.forward in eval mode (model_components/renderers.py:233-268, combine_rgb :103-148)."""
-    rgb = torch.nan_to_num(rgb)
+def rgb_render(rgb: Tensor, weights: Tensor, background: Optional[Tensor], training: bool = False) -> Tensor:
+    """RGBRenderer.forward (model_components/renderers.py:233-268, combine_rgb :103-148): in eval mode nan_to_num of the
+    samples' rgb and a clamp of the result to [0, 1]; in training mode neither."""
+    if not training:
+        rgb = torch.nan_to_num(rgb)
     comp = torch.sum(weights * rgb, dim=-2)
-    if background is None:  # "random": as if black, no blending
-        return comp
-    acc = torch.sum(weights, dim=-2)
-    return comp + background * (1.0 - acc)
+    if background is not None:  # None is "random": as if black, no blending
+        comp = comp + background * (1.0 - torch.sum(weights, dim=-2))
+    return comp if training else torch.clamp(comp, min=0.0, max=1.0)
 
 
 def depth_expected(weights: Tensor, starts: Tensor, ends: Tensor) -> Tensor:

@@ -134,9 +134,13 @@ class FakeBackend(B200Backend):
 
     @torch.no_grad()
     def frustum_positions(self, origins, directions, bins_e, aabb=None):
-        assert aabb is None
         n = bins_e.shape[0]
-        return S.frustum_positions(origins.reshape(n, 3), directions.reshape(n, 3), bins_e[:, :-1, None], bins_e[:, 1:, None])
+        p = S.frustum_positions(origins.reshape(n, 3), directions.reshape(n, 3), bins_e[:, :-1, None], bins_e[:, 1:, None])
+        return p if aabb is None else S.normalized_positions(p, aabb.float())
+
+    @torch.no_grad()
+    def density_rgb_heads(self, raw):
+        return torch.exp(raw[..., :1]), torch.sigmoid(raw[..., 1:])
 
     @torch.no_grad()
     def hashgrid_fwd(self, g, table, x, scalings=None, want_indices=False):
@@ -217,13 +221,20 @@ class FakeBackend(B200Backend):
         w = weights.reshape(n, s, 1)
         out = {}
         if values is not None:
-            out["values"] = (w * values.reshape(n, s, -1)).sum(dim=-2)
+            if values.shape[-1] > 64:
+                raise ValueError("at most 64 value channels")
+            v = values.reshape(n, s, values.shape[-1])
+            out["values"] = (w * (torch.nan_to_num(v) if value_nan_to_num else v)).sum(dim=-2)
+            if background is not None:
+                out["values"] = out["values"] + torch.tensor(background, dtype=torch.float32) * (1.0 - w.sum(dim=-2))
         if want_accumulation:
             out["accumulation"] = w.sum(dim=-2)
         if depth_method == "simple":
             out["depth"] = (w * (starts.reshape(n, s, 1) + ends.reshape(n, s, 1)) / 2).sum(dim=-2)
         elif depth_method == "median":
             out["depth"] = S.depth_median(w, starts.reshape(n, s, 1), ends.reshape(n, s, 1))
+        elif depth_method == "expected":
+            out["depth"] = S.depth_expected(w, starts.reshape(n, s, 1), ends.reshape(n, s, 1))
         elif depth_method is not None:
             raise NotImplementedError(depth_method)
         return out

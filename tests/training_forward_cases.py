@@ -318,14 +318,15 @@ def resample_bits(cdf, inds, bins, uu):
     return b0 + t * (b1 - b0)
 
 
-def check_pdf(out, w, bins, S_new, rand, hp, what):
+def check_pdf(out, w, bins, S_new, rand, hp, what, u=None):
     """cdf per entry (cdf_reference); inds bit for bit = torch.searchsorted(kernel cdf, u, right=True) (the kernel's
-    binary search is torch's); new bins bit for bit from the kernel's cdf and indices."""
+    binary search is torch's); new bins bit for bit from the kernel's cdf and indices.  `u` [n, S_new + 1]: the
+    quantiles when no `rand` is drawn (eval mode)."""
     nb, cdf, inds = out
     ref, tol = cdf_reference(w, hp)
     worst = _ratio(cdf, ref, tol, what + " cdf")
     kc = cdf.detach().cpu().float().contiguous()
-    uu = pdf_quantiles(S_new, rand)
+    uu = pdf_quantiles(S_new, rand) if u is None else u
     _bits_equal(inds, torch.searchsorted(kc, uu, right=True).int(), what + " inds")
     _bits_equal(nb, resample_bits(kc, inds.cpu(), bins.float().cpu().reshape(kc.shape), uu), what + " bins")
     return worst
@@ -798,11 +799,11 @@ class Recorder:
     """Wraps the listed methods of one backend instance; every call's arguments and results are copied (the module walk
     edits some tensors in place afterwards, e.g. the last edge moved to the sky)."""
 
-    def __init__(self, be):
-        self.be, self.calls = be, []
+    def __init__(self, be, methods=RECORDED):
+        self.be, self.methods, self.calls = be, tuple(methods), []
 
     def __enter__(self):
-        for name in RECORDED:
+        for name in self.methods:
             orig = getattr(self.be, name)
 
             def wrap(*a, _orig=orig, _name=name, **k):
@@ -814,7 +815,7 @@ class Recorder:
         return self
 
     def __exit__(self, *exc):
-        for name in RECORDED:
+        for name in self.methods:
             delattr(self.be, name)
 
 
@@ -824,9 +825,9 @@ def training_scene(dev, n_actors=8, seed=0):
     return cfg, trajs, scene.make_params(cfg, seed=seed, beta=3.0, sdf_bias=0.6, trajectories=trajs)
 
 
-def record_training_step(dev, n_cam, n_lidar, seed=0):
+def record_training_step(dev, n_cam, n_lidar, seed=0, methods=RECORDED):
     """model.train(); get_nff_outputs(fused=False) on a seeded scene with actors, then backward of a simple loss (so that
-    mlp_dgrad is called too); returns (cfg, params, backend, recorded calls)."""
+    mlp_dgrad is called too); returns (cfg, params, backend, the recorded calls of `methods`)."""
     from neurad_studio_b200 import nerfstudio_api as NA
 
     cfg, trajs, params = training_scene(dev, seed=seed)
@@ -847,7 +848,7 @@ def record_training_step(dev, n_cam, n_lidar, seed=0):
     try:
         be = model._bind()
         torch.manual_seed(seed)
-        with Recorder(be) as rec:
+        with Recorder(be, methods) as rec:
             out = model.get_nff_outputs(rb, fused=False)
             (out["features"].square().mean() + out["depth"].mean() * 1e-3).backward()
     finally:
